@@ -110,8 +110,10 @@ struct workspace {
   size_t cap_n = 0;  // scalars the buffers are sized for
   void* scalars = nullptr;
   int32_t* digits = nullptr;
-  uint32_t *counts = nullptr, *start = nullptr, *cursor = nullptr, *blocksums = nullptr;
-  uint64_t* entries = nullptr;
+  uint32_t *sortctl = nullptr, *start = nullptr;
+  uint64_t *entries = nullptr, *entries_tmp = nullptr;
+  unsigned long long* look = nullptr;  // look-back words of the radix passes
+  uint32_t sort_epoch = 0;             // last look-back tag used on these buffers
   void *buckets = nullptr, *parts = nullptr, *rparts = nullptr, *sumscratch = nullptr;
   uint32_t* pkeys = nullptr;
   uint32_t* heavy = nullptr;
@@ -129,7 +131,7 @@ struct workspace {
   cudaEvent_t busy = nullptr;
   void release() {
     if (busy) cudaEventDestroy(busy);
-    void* ptrs[] = {scalars, digits, counts, start, cursor, blocksums, entries, buckets,
+    void* ptrs[] = {scalars, digits, sortctl, start, entries, entries_tmp, look, buckets,
                     parts, rparts, sumscratch, pkeys, heavy, hparts, d_out, idx32};
     for (void* p : ptrs)
       if (p) cudaFree(p);
@@ -194,7 +196,8 @@ struct ck_ctx {
 
 // ---- optional per-stage device timing + launch accounting (for bench.py's roofline) ---------
 enum { ST_DIGITS = 0, ST_SORT, ST_ACCUMULATE, ST_FIXUP, ST_REDUCE, ST_COUNT };
-const int STAGE_KERNELS[ST_COUNT] = {1, 4, 1, 3, 2};  // reduce: merge + final (+ one per level, added per call)
+// sort: the bucket starts (+ one per radix pass, added per call); reduce: merge + final (+ one per level, likewise)
+const int STAGE_KERNELS[ST_COUNT] = {1, 1, 1, 3, 2};
 struct profile_state {
   std::mutex mu;
   bool enabled = false;
@@ -300,11 +303,14 @@ int ensure_workspace(ck_ctx& ck, workspace& w, size_t n, size_t out_slots) {
     w.out_slots = out_slots;
   }
   if (n <= w.cap_n) return B200_OK;
+  // entries, bucket starts and the sort's positions are 32-bit (table indices 31-bit)
+  if (n * (size_t)ck.W > 0x7FFFFFFFu)
+    return fail(B200_E_RANGE, "%zu scalars x %d windows exceed 2^31 bucket entries", n, ck.W);
   // grow: release the size-dependent buffers and reallocate (after draining any asynchronous
   // *_dev work that may still be using them)
   CU(cudaDeviceSynchronize());
-  void** szbufs[] = {&w.scalars, (void**)&w.digits, (void**)&w.entries, &w.parts, (void**)&w.pkeys,
-                     (void**)&w.heavy, &w.hparts};
+  void** szbufs[] = {&w.scalars, (void**)&w.digits, (void**)&w.entries, (void**)&w.entries_tmp, (void**)&w.look,
+                     &w.parts, (void**)&w.pkeys, (void**)&w.heavy, &w.hparts};
   for (void** p : szbufs)
     if (*p) {
       cudaFree(*p);
@@ -319,13 +325,17 @@ int ensure_workspace(ck_ctx& ck, workspace& w, size_t n, size_t out_slots) {
   CU(cudaMalloc(&w.scalars, n * 32));
   CU(cudaMalloc((void**)&w.digits, entries * sizeof(int32_t)));
   CU(cudaMalloc((void**)&w.entries, entries * sizeof(uint64_t)));
+  CU(cudaMalloc((void**)&w.entries_tmp, entries * sizeof(uint64_t)));
+  // zeroed once: a zero word carries no valid tag (see msm_sort.cuh)
+  const size_t look_bytes = (entries + SORT_TILE - 1) / SORT_TILE * SORT_BINS * sizeof(unsigned long long);
+  CU(cudaMalloc((void**)&w.look, look_bytes));
+  CU(cudaMemset(w.look, 0, look_bytes));
+  w.sort_epoch = 0;
   CU(cudaMalloc(&w.parts, 2 * nseg * XYZZ_BYTES));
   CU(cudaMalloc((void**)&w.pkeys, 2 * nseg * sizeof(uint32_t)));
-  if (!w.counts) {
-    CU(cudaMalloc((void**)&w.counts, K * 4));
+  if (!w.sortctl) {
+    CU(cudaMalloc((void**)&w.sortctl, SORT_CTL_WORDS * 4));
     CU(cudaMalloc((void**)&w.start, (K + 1) * 4));
-    CU(cudaMalloc((void**)&w.cursor, K * 4));
-    CU(cudaMalloc((void**)&w.blocksums, 4096 * 4));
     CU(cudaMalloc(&w.buckets, K * XYZZ_BYTES));
     // chunk partials of the running-sum reduce, or [G][NR+NC] row/column sums + [G][2] of the
     // two-level reduce (NR + NC <= 2 * sqrt(2B) + 1 <= B / m + 514)
@@ -358,15 +368,17 @@ msm_plan make_plan(ck_ctx& ck, workspace& ws, size_t base_offset, size_t n) {
   p.heavy_cap = ws.heavy_cap;
   p.hparts = ws.hparts;
   p.digits = ws.digits;
-  p.counts = ws.counts;
+  p.sortctl = ws.sortctl;
+  p.sp = make_sort_plan((uint64_t)ck.G * ck.B);
+  p.sort_tag = 0;  // set per call by enqueue_msm
+  p.look = ws.look;
   p.start = ws.start;
-  p.cursor = ws.cursor;
   p.entries = ws.entries;
+  p.entries_tmp = ws.entries_tmp;
   p.buckets = ws.buckets;
   p.parts = ws.parts;
   p.pkeys = ws.pkeys;
   p.rparts = ws.rparts;
-  p.blocksums = ws.blocksums;
   return p;
 }
 
@@ -375,7 +387,8 @@ int enqueue_msm(ck_ctx& ck, workspace& ws, size_t base_offset, const void* d_sca
                 void* d_out, cudaStream_t s, int small_elem_bytes = 0, bool blinded = false,
                 bool digits_done = false, const msm_peer* peer = nullptr, bool profile_ok = true) {
   // blinded: d_scalars holds n-1 vector entries followed by r, whose base is h
-  // digits_done: ws.digits / ws.counts were already filled chunk by chunk (b200_witness_append)
+  // digits_done: ws.digits and the radix histograms of ws.sortctl were already filled chunk by chunk
+  // (b200_witness_append, the chunked upload of b200_commit)
   const field_ops* sops = ops_for_field(CURVES[ck.curve].scalar_fid);
   const field_ops* bops = ops_for_field(CURVES[ck.curve].base_fid);
   {
@@ -397,9 +410,18 @@ int enqueue_msm(ck_ctx& ck, workspace& ws, size_t base_offset, const void* d_sca
   msm_plan p = make_plan(ck, ws, base_offset, n);
   if (peer) p.peer = *peer;
   if (blinded) p.blind_i = n - 1;
-  size_t K = (size_t)ck.G * ck.B;
-  if (!digits_done) CU(cudaMemsetAsync(p.counts, 0, K * 4, s));
+  // histograms and tile counters; only the tile counters when the digit stage already ran
+  if (!digits_done) CU(cudaMemsetAsync(p.sortctl, 0, SORT_CTL_WORDS * 4, s));
+  else CU(cudaMemsetAsync(p.sortctl + SORT_PASSES_MAX * SORT_BINS, 0, SORT_PASSES_MAX * 4, s));
   CU(cudaMemsetAsync(p.heavy, 0, 4, s));
+  // look-back tags: fresh for every pass of every call on these buffers; the (practically unreachable) wrap of the
+  // 31-bit tag space re-zeroes the words so that no stale word can carry a live tag
+  if (ws.sort_epoch > 0x7FFFFFFFu - SORT_PASSES_MAX) {
+    CU(cudaMemsetAsync(ws.look, 0, (ws.cap_n * (size_t)ck.W + SORT_TILE - 1) / SORT_TILE * SORT_BINS * 8, s));
+    ws.sort_epoch = 0;
+  }
+  p.sort_tag = ws.sort_epoch + 1;
+  ws.sort_epoch += (uint32_t)p.sp.passes;
   std::lock_guard<std::mutex> plk(g_prof.mu);
   const bool prof = g_prof.enabled && profile_ok;  // (the stage events belong to the library's own device)
   const int pset = g_prof.next;
@@ -422,8 +444,7 @@ int enqueue_msm(ck_ctx& ck, workspace& ws, size_t base_offset, const void* d_sca
   else
     sops->digits(s, d_scalars, p);
   STAGE_MARK(ST_SORT);
-  msm_scan(s, p);
-  msm_scatter(s, p);
+  const int sort_launches = msm_sort(s, p);
   STAGE_MARK(ST_ACCUMULATE);
   bops->accumulate(s, ck.tables, p);
   STAGE_MARK(ST_FIXUP);
@@ -434,6 +455,7 @@ int enqueue_msm(ck_ctx& ck, workspace& ws, size_t base_offset, const void* d_sca
 #undef STAGE_MARK
   if (prof) g_prof.pending[pset] = true;
   for (int i = 0; i < ST_COUNT; i++) g_prof.launches += STAGE_KERNELS[i];
+  g_prof.launches += sort_launches - STAGE_KERNELS[ST_SORT];  // the radix passes
   g_prof.launches += (ck.c - 1 + 3) / 4 - 1;  // the hierarchical reduction launches one kernel per level below the top
   CU(cudaGetLastError());
   return ws_release(ws, s);
@@ -939,7 +961,7 @@ static int msm_host(ck_ctx& ck, size_t base_offset, const void* scalars, size_t 
     CU(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
     CU(cudaEventRecord(ev, s));  // order the side stream after earlier users of this workspace
     CU(cudaStreamWaitEvent(side, ev, 0));
-    CU(cudaMemsetAsync(p.counts, 0, (size_t)ck.G * ck.B * 4, side));
+    CU(cudaMemsetAsync(p.sortctl, 0, SORT_CTL_WORDS * 4, side));
     const size_t per = (n + h2d_chunks - 1) / h2d_chunks;
     auto piece = [&](const void* src, size_t lo, size_t hi) -> int {
       CU(cudaMemcpyAsync((char*)W.scalars + 32 * lo, src, 32 * (hi - lo), cudaMemcpyHostToDevice, s));

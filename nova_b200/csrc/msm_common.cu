@@ -1,208 +1,50 @@
-// Field-independent MSM stages: histogram scan and counting-sort scatter.
+// Field-independent MSM stages: the integer-scalar digit kernel and the radix sort of the entries.
 #include "ops.cuh"
 #include "msm_kernels.cuh"
 
 namespace nova {
 
-// ------------------------------------------------------------------------------------------
-// exclusive scan of counts[K] -> start[K+1], cursor[K]   (3 small kernels, K <= 2^22 * G)
-// ------------------------------------------------------------------------------------------
-constexpr int SCAN_BLOCK = 1024;
-constexpr int SCAN_ITEMS = 4;  // per thread -> 4096 per block
-
-__global__ void __launch_bounds__(SCAN_BLOCK) k_scan_block(const uint32_t* __restrict__ in,
-                                                           uint32_t* __restrict__ out,
-                                                           uint32_t* __restrict__ blocksums,
-                                                           uint32_t K) {
-  __shared__ uint32_t warp_tot[32];
-  uint32_t base = blockIdx.x * (SCAN_BLOCK * SCAN_ITEMS) + threadIdx.x * SCAN_ITEMS;
-  uint32_t v[SCAN_ITEMS], tot = 0;
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; k++) {
-    v[k] = (base + k < K) ? in[base + k] : 0;
-    tot += v[k];
-  }
-  // warp inclusive scan of tot
-  uint32_t inc = tot;
-  int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t o = __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc += o;
-  }
-  if (lane == 31) warp_tot[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    uint32_t w = warp_tot[lane];
-    uint32_t winc = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t o = __shfl_up_sync(0xffffffffu, winc, d);
-      if (lane >= d) winc += o;
-    }
-    warp_tot[lane] = winc - w;  // exclusive
-    if (lane == 31) blocksums[blockIdx.x] = winc;
-  }
-  __syncthreads();
-  uint32_t excl = inc - tot + warp_tot[wid];
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; k++) {
-    if (base + k < K) out[base + k] = excl;
-    excl += v[k];
-  }
-}
-
-__global__ void __launch_bounds__(SCAN_BLOCK) k_scan_sums(uint32_t* blocksums, uint32_t nblocks) {
-  // single block, exclusive scan in place; nblocks <= SCAN_BLOCK*SCAN_ITEMS
-  __shared__ uint32_t warp_tot[32];
-  uint32_t base = threadIdx.x * SCAN_ITEMS;
-  uint32_t v[SCAN_ITEMS], tot = 0;
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; k++) {
-    v[k] = (base + k < nblocks) ? blocksums[base + k] : 0;
-    tot += v[k];
-  }
-  uint32_t inc = tot;
-  int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    uint32_t o = __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc += o;
-  }
-  if (lane == 31) warp_tot[wid] = inc;
-  __syncthreads();
-  if (wid == 0) {
-    uint32_t w = warp_tot[lane], winc = w;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      uint32_t o = __shfl_up_sync(0xffffffffu, winc, d);
-      if (lane >= d) winc += o;
-    }
-    warp_tot[lane] = winc - w;
-  }
-  __syncthreads();
-  uint32_t excl = inc - tot + warp_tot[wid];
-#pragma unroll
-  for (int k = 0; k < SCAN_ITEMS; k++) {
-    if (base + k < nblocks) blocksums[base + k] = excl;
-    excl += v[k];
-  }
-}
-
-__global__ void __launch_bounds__(256) k_scan_add(uint32_t* __restrict__ start,
-                                                  uint32_t* __restrict__ cursor,
-                                                  const uint32_t* __restrict__ counts,
-                                                  const uint32_t* __restrict__ blocksums,
-                                                  uint32_t K, uint32_t* __restrict__ heavy,
-                                                  uint32_t heavy_min, uint32_t heavy_cap) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= K) return;
-  uint32_t s = start[i] + blocksums[i / (SCAN_BLOCK * SCAN_ITEMS)];
-  start[i] = s;
-  cursor[i] = s;
-  uint32_t cnt = counts[i];
-  if (i == K - 1) start[K] = s + cnt;
-  if (cnt > heavy_min) {  // at most M / heavy_min such keys, which is what heavy_cap is sized for
-    uint32_t slot = atomicAdd(&heavy[0], 1u);
-    if (slot < heavy_cap) heavy[1 + slot] = i;
-  }
-}
-
-// integer scalars (msm.rs:469-503): unsigned little-endian elements of 1/2/4/8 bytes -> the same
-// signed c-bit digit stream as k_digits; zero scalars produce no entries (msm.rs:512,545)
-__global__ void __launch_bounds__(256) k_digits_small(const void* __restrict__ scalars,
-                                                      int elem_bytes, size_t n, int c, int W, int G,
-                                                      uint32_t B, int32_t* __restrict__ digits,
-                                                      uint32_t* __restrict__ counts) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool live = i < n;  // no early exit: the whole warp takes part in count_key
-  uint64_t v64 = 0;
-  if (live) switch (elem_bytes) {
-    case 1: v64 = ((const uint8_t*)scalars)[i]; break;
-    case 2: v64 = ((const uint16_t*)scalars)[i]; break;
-    case 4: v64 = ((const uint32_t*)scalars)[i]; break;
-    default: v64 = ((const uint64_t*)scalars)[i]; break;
-  }
-  const uint32_t half = 1u << (c - 1);
-  const uint64_t mask = (1ull << c) - 1;
-  uint32_t carry = 0;
-  for (int w = 0; w < W; w++) {
-    int bit = w * c;
-    uint32_t v = bit < 64 ? (uint32_t)((v64 >> bit) & mask) : 0u;
-    v += carry;
-    int32_t dgt;
-    if (v > half) {
-      dgt = (int32_t)v - (int32_t)(1u << c);
-      carry = 1;
-    } else {
-      dgt = (int32_t)v;
-      carry = 0;
-    }
-    if (live) digits[(size_t)w * n + i] = dgt;
-    uint32_t key = NO_KEY;
-    if (dgt != 0) {
-      uint32_t mag = dgt < 0 ? (uint32_t)(-dgt) : (uint32_t)dgt;
-      key = (uint32_t)(w % G) * B + (mag - 1);
-    }
-    count_key(counts, key);
-  }
-}
-
-// ------------------------------------------------------------------------------------------
-// scatter
-// ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_scatter(const int32_t* __restrict__ digits, size_t n,
-                                                 int W, int G, uint32_t B, size_t n_ck,
-                                                 size_t base_offset, size_t blind_i, size_t h_index,
-                                                 uint32_t* __restrict__ cursor,
-                                                 uint64_t* __restrict__ entries) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int w = blockIdx.y;
-  int32_t dgt = i < n ? digits[(size_t)w * n + i] : 0;  // no early exit (warp-wide match below)
-  uint32_t sign = dgt < 0 ? 1u : 0u;
-  uint32_t mag = sign ? (uint32_t)(-dgt) : (uint32_t)dgt;
-  uint32_t key = dgt != 0 ? (uint32_t)(w % G) * B + (mag - 1) : NO_KEY;
-  // slot reservation; warps that hold repeated keys aggregate (see count_key): one atomic per
-  // distinct key, lanes take consecutive slots by their rank inside the group
-  uint32_t pos;
-  if (!warp_has_repeats(key)) {
-    if (key == NO_KEY) return;
-    pos = atomicAdd(&cursor[key], 1u);
-  } else {
-    unsigned peers = __match_any_sync(0xFFFFFFFFu, key);
-    if (key == NO_KEY) return;
-    unsigned lane = threadIdx.x & 31u, leader = (unsigned)(__ffs(peers) - 1);
-    uint32_t base = 0;
-    if (lane == leader) base = atomicAdd(&cursor[key], (uint32_t)__popc(peers));
-    base = __shfl_sync(peers, base, leader);
-    pos = base + (uint32_t)__popc(peers & ((1u << lane) - 1u));
-  }
-  // the blinding scalar r rides along as one more (scalar, base) pair whose base is h
-  size_t bi = (i == blind_i) ? h_index : base_offset + i;
-  uint32_t idx = (uint32_t)((size_t)(w / G) * n_ck + bi);
-  entries[pos] = ((uint64_t)key << 32) | ((uint64_t)sign << 31) | idx;
-}
-
-void msm_scan(cudaStream_t s, const msm_plan& p) {
-  uint32_t K = (uint32_t)p.G * p.B;
-  uint32_t per_block = SCAN_BLOCK * SCAN_ITEMS;
-  uint32_t nblocks = (K + per_block - 1) / per_block;
-  k_scan_block<<<nblocks, SCAN_BLOCK, 0, s>>>(p.counts, p.start, p.blocksums, K);
-  k_scan_sums<<<1, SCAN_BLOCK, 0, s>>>(p.blocksums, nblocks);
-  k_scan_add<<<(K + 255) / 256, 256, 0, s>>>(p.start, p.cursor, p.counts, p.blocksums, K, p.heavy,
-                                             p.heavy_min, p.heavy_cap);
-}
-
 void msm_digits_small(cudaStream_t s, const void* scalars, int elem_bytes, const msm_plan& p) {
-  k_digits_small<<<(unsigned)((p.n + 255) / 256), 256, 0, s>>>(scalars, elem_bytes, p.n, p.c, p.W,
-                                                               p.G, p.B, p.digits, p.counts);
+  size_t blocks = (p.n + 255) / 256;
+  unsigned grid = (unsigned)(blocks < SORT_HIST_BLOCKS ? blocks : SORT_HIST_BLOCKS);
+  k_digits_small<<<grid, 256, 0, s>>>(scalars, elem_bytes, p.n, p.c, p.W, p.G, p.B, p.digits, p.sortctl, p.sp);
 }
 
-void msm_scatter(cudaStream_t s, const msm_plan& p) {
-  dim3 grid((unsigned)((p.n + 255) / 256), (unsigned)p.W);
-  k_scatter<<<grid, 256, 0, s>>>(p.digits, p.n, p.W, p.G, p.B, p.n_ck, p.base_offset, p.blind_i,
-                                 p.h_index, p.cursor,
-                                 p.entries);
+sort_args make_sort_args(const msm_plan& p) {
+  sort_args a;
+  a.n = (uint32_t)p.n;
+  a.count = (uint32_t)(p.n * (size_t)p.W);
+  a.W = p.W;
+  a.G = p.G;
+  a.B = p.B;
+  a.n_ck = (uint32_t)p.n_ck;
+  a.base_offset = (uint32_t)p.base_offset;
+  a.blind_i = p.blind_i == SIZE_MAX ? NO_KEY : (uint32_t)p.blind_i;
+  a.h_index = (uint32_t)p.h_index;
+  a.sp = p.sp;
+  return a;
+}
+
+// the radix passes (pass 0 reads the digits; the last pass writes p.entries), then the bucket starts;
+// returns the number of kernels launched
+int msm_sort(cudaStream_t s, const msm_plan& p) {
+  const sort_args a = make_sort_args(p);
+  const unsigned tiles = (unsigned)((a.count + SORT_TILE - 1) / SORT_TILE);
+  const int P = p.sp.passes;
+  const uint64_t* in = nullptr;
+  for (int pass = 0; pass < P; pass++) {
+    uint64_t* out = ((P - 1 - pass) & 1) ? p.entries_tmp : p.entries;
+    if (pass == 0)
+      k_sort_pass<true><<<tiles, SORT_THREADS, 0, s>>>(p.digits, nullptr, out, a, 0, p.sortctl, p.look, p.sort_tag);
+    else
+      k_sort_pass<false><<<tiles, SORT_THREADS, 0, s>>>(nullptr, in, out, a, pass, p.sortctl, p.look,
+                                                        p.sort_tag + (uint32_t)pass);
+    in = out;
+  }
+  const uint32_t K = (uint32_t)p.G * p.B;
+  k_sort_starts<<<(K + 1 + SORT_THREADS - 1) / SORT_THREADS, SORT_THREADS, 0, s>>>(
+      p.entries, p.sortctl, p.sp, K, p.start, p.heavy, p.heavy_min, p.heavy_cap);
+  return P + 1;
 }
 
 }  // namespace nova

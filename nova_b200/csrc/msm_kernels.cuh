@@ -12,9 +12,9 @@
 //
 // Pipeline (all on one stream, no host sync):
 //   k_digits      scalar (Montgomery) -> canonical -> sign-fold (s > p/2 => p-s, flip) ->
-//                 signed c-bit digits; histogram of bucket keys            [msm.rs:247-252 idea]
-//   scan          exclusive prefix sum of the histogram
-//   k_scatter     counting-sort scatter of (key, sign, table index) entries
+//                 signed c-bit digits; per-pass radix histograms of the bucket keys  [msm.rs:247-252 idea]
+//   k_sort_pass   stable LSD radix sort of the (key, sign, table index) entries by key (msm_sort.cuh)
+//   k_sort_starts bucket starts and the heavy-bucket list
 //   k_accumulate  one thread per L consecutive sorted entries: XYZZ mixed adds
 //                 (msm.rs:126-165); interior runs go straight to their bucket, the first/last
 //                 run of a segment to a boundary-partial list
@@ -25,6 +25,7 @@
 #include <cuda_runtime.h>
 #include "curve29.cuh"
 #include "coop.cuh"
+#include "msm_sort.cuh"
 
 namespace nova {
 
@@ -59,15 +60,17 @@ struct msm_plan {
   int m;               // buckets per reduce chunk
   // workspace (device)
   int32_t* digits;     // [W][n]
-  uint32_t* counts;    // [K]     K = G*B
+  uint32_t* sortctl;   // [SORT_CTL_WORDS]: per-pass radix histograms, then the per-pass tile counters
+  sort_plan sp;        // radix passes over the keys [0, K), K = G*B
+  uint32_t sort_tag;   // look-back tag of pass 0 (pass p uses sort_tag + p)
+  unsigned long long* look;  // [ceil(n*W / SORT_TILE) * SORT_BINS] look-back words
   uint32_t* start;     // [K+1]
-  uint32_t* cursor;    // [K]
-  uint64_t* entries;   // [n*W]
+  uint64_t* entries;   // [n*W]   sorted by key
+  uint64_t* entries_tmp;  // [n*W] the other buffer of the radix passes
   void* buckets;       // [K] xyzz
   void* parts;         // [2*nseg_max] xyzz
   uint32_t* pkeys;     // [2*nseg_max]
   void* rparts;        // [G*T] xyzz, T = B/m
-  uint32_t* blocksums; // scan scratch
   uint32_t* heavy;     // [0] = count, [1..] = keys whose bucket spans > heavy_min entries
   uint32_t heavy_min;  // entries; such buckets are joined by k_fixup_heavy1/2
   uint32_t heavy_cap;  // capacity of the heavy list
@@ -78,83 +81,68 @@ struct msm_plan {
 // ------------------------------------------------------------------------------------------
 // digits + histogram   (templated on the SCALAR field)
 // ------------------------------------------------------------------------------------------
-// Warp-aggregated bucket counting for skewed scalars (bits, padding, one value repeated a million
-// times): lanes holding the same key elect one leader that adds the group's size, which divides
-// the atomics on a hot counter by up to 32.  MATCH.ANY is slow enough to cost ~0.1 ms per 2^20
-// uniform MSM, so a warp only takes that path when two NEIGHBOURING lanes hold the same key (one
-// shuffle + one vote): uniform digits practically never do, a bucket that owns >= 10 % of the
-// entries almost always does.  `key` = NO_KEY for lanes without an entry; all 32 lanes must call.
-constexpr uint32_t NO_KEY = 0xFFFFFFFFu;
-__device__ __forceinline__ bool warp_has_repeats(uint32_t key) {
-  uint32_t next = __shfl_down_sync(0xFFFFFFFFu, key, 1);
-  return __any_sync(0xFFFFFFFFu, key != NO_KEY && key == next && (threadIdx.x & 31u) != 31u);
-}
-__device__ __forceinline__ void count_key(uint32_t* counts, uint32_t key) {
-  if (!warp_has_repeats(key)) {
-    if (key != NO_KEY) atomicAdd(&counts[key], 1u);
-    return;
-  }
-  unsigned peers = __match_any_sync(0xFFFFFFFFu, key);
-  if (key != NO_KEY && (threadIdx.x & 31u) == (unsigned)(__ffs(peers) - 1))
-    atomicAdd(&counts[key], (uint32_t)__popc(peers));
-}
-
 // Processes scalars [i0, i1) of a vector of n (the digit array is [W][n]): a whole MSM passes
 // (0, n); the streamed witness hand-off (b200_witness_append) passes each chunk as it arrives.
+// Grid-stride over blocks of 256 scalars; the block's radix histograms are added to hist at the end.
 template <class S>
 __global__ void __launch_bounds__(256) k_digits(const void* __restrict__ scalars, size_t i0, size_t i1,
                                                 size_t n, int c, int W, int G, uint32_t B,
                                                 int32_t* __restrict__ digits,
-                                                uint32_t* __restrict__ counts) {
-  size_t i = i0 + (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  const bool live = i < i1;  // no early exit: the whole warp takes part in count_key
-  fe_t s = live ? fe_from_mont<S>(fe_load(scalars, i)) : fe_zero<S>();
-  // sign fold: use p - s when that is the smaller integer (msm.rs:1-8 "signed scalar
-  // decomposition"); small negative witness values then cost one bucket add, not W.
-  uint32_t p[8], t[8];
-  load_p<S>(p);
-  bool neg = false;
-  if (!fe_is_zero(s)) {
-    sub8(t, p, s.l);  // p - s, never borrows
-    // compare t < s  <=> p - s < s
-    uint32_t d[8];
-    uint32_t lt = sub8(d, t, s.l);
-    if (lt) {
-      neg = true;
+                                                uint32_t* __restrict__ hist, const sort_plan sp) {
+  __shared__ uint32_t s_hist[SORT_PASSES_MAX * SORT_BINS];
+  sort_hist_clear(s_hist);
+  for (size_t blk = i0 + (size_t)blockIdx.x * blockDim.x; blk < i1; blk += (size_t)gridDim.x * blockDim.x) {
+    size_t i = blk + threadIdx.x;
+    const bool live = i < i1;  // no early exit: the whole warp takes part in sort_hist_count
+    fe_t s = live ? fe_from_mont<S>(fe_load(scalars, i)) : fe_zero<S>();
+    // sign fold: use p - s when that is the smaller integer (msm.rs:1-8 "signed scalar
+    // decomposition"); small negative witness values then cost one bucket add, not W.
+    uint32_t p[8], t[8];
+    load_p<S>(p);
+    bool neg = false;
+    if (!fe_is_zero(s)) {
+      sub8(t, p, s.l);  // p - s, never borrows
+      // compare t < s  <=> p - s < s
+      uint32_t d[8];
+      uint32_t lt = sub8(d, t, s.l);
+      if (lt) {
+        neg = true;
 #pragma unroll
-      for (int k = 0; k < 8; k++) s.l[k] = t[k];
+        for (int k = 0; k < 8; k++) s.l[k] = t[k];
+      }
+    }
+    const uint32_t half = 1u << (c - 1);
+    const uint32_t mask = (1u << c) - 1;
+    uint32_t carry = 0;
+    for (int w = 0; w < W; w++) {
+      int bit = w * c;
+      int limb = bit >> 5, sh = bit & 31;
+      uint32_t v = 0;
+      if (limb < 8) {
+        uint64_t two = s.l[limb];
+        if (limb + 1 < 8) two |= (uint64_t)s.l[limb + 1] << 32;
+        v = (uint32_t)(two >> sh) & mask;
+      }
+      v += carry;
+      int32_t dgt;
+      if (v > half) {  // digits in [-(half-1), half]
+        dgt = (int32_t)v - (int32_t)(1u << c);
+        carry = 1;
+      } else {
+        dgt = (int32_t)v;
+        carry = 0;
+      }
+      if (neg) dgt = -dgt;
+      if (live) digits[(size_t)w * n + i] = dgt;
+      uint32_t key = NO_KEY;
+      if (dgt != 0) {
+        uint32_t mag = dgt < 0 ? (uint32_t)(-dgt) : (uint32_t)dgt;
+        key = (uint32_t)(w % G) * B + (mag - 1);
+      }
+      sort_hist_count(s_hist, key, sp);
     }
   }
-  const uint32_t half = 1u << (c - 1);
-  const uint32_t mask = (1u << c) - 1;
-  uint32_t carry = 0;
-  for (int w = 0; w < W; w++) {
-    int bit = w * c;
-    int limb = bit >> 5, sh = bit & 31;
-    uint32_t v = 0;
-    if (limb < 8) {
-      uint64_t two = s.l[limb];
-      if (limb + 1 < 8) two |= (uint64_t)s.l[limb + 1] << 32;
-      v = (uint32_t)(two >> sh) & mask;
-    }
-    v += carry;
-    int32_t dgt;
-    if (v > half) {  // digits in [-(half-1), half]
-      dgt = (int32_t)v - (int32_t)(1u << c);
-      carry = 1;
-    } else {
-      dgt = (int32_t)v;
-      carry = 0;
-    }
-    if (neg) dgt = -dgt;
-    if (live) digits[(size_t)w * n + i] = dgt;
-    uint32_t key = NO_KEY;
-    if (dgt != 0) {
-      uint32_t mag = dgt < 0 ? (uint32_t)(-dgt) : (uint32_t)dgt;
-      key = (uint32_t)(w % G) * B + (mag - 1);
-    }
-    count_key(counts, key);
-  }
+  sort_hist_flush(s_hist, hist, sp);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -146,8 +146,7 @@ inline const field_ops* ops_for_field(int fid) {
 }
 
 // field-independent MSM stages (msm_common.cu)
-void msm_scan(cudaStream_t, const msm_plan&);
-void msm_scatter(cudaStream_t, const msm_plan&);
+int msm_sort(cudaStream_t, const msm_plan&);  // returns the number of kernels launched
 void msm_digits_small(cudaStream_t, const void* scalars, int elem_bytes, const msm_plan&);
 
 }  // namespace nova

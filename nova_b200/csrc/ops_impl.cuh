@@ -45,8 +45,9 @@ struct ops_impl {
   static void digits_range(cudaStream_t s, const void* scalars, size_t i0, size_t i1, const msm_plan& p) {
     if (i1 <= i0) return;
     int block = 256;
-    int grid = (int)((i1 - i0 + block - 1) / block);
-    k_digits<F><<<grid, block, 0, s>>>(scalars, i0, i1, p.n, p.c, p.W, p.G, p.B, p.digits, p.counts);
+    size_t blocks = (i1 - i0 + block - 1) / block;
+    int grid = (int)(blocks < SORT_HIST_BLOCKS ? blocks : SORT_HIST_BLOCKS);
+    k_digits<F><<<grid, block, 0, s>>>(scalars, i0, i1, p.n, p.c, p.W, p.G, p.B, p.digits, p.sortctl, p.sp);
   }
   static void expand_key(cudaStream_t s, void* tables, size_t n_ck, int ntables, int shift) {
     int block = 128;
