@@ -448,6 +448,27 @@ int b200_poly_eval_many_dev(int field_id, const void* const* d_polys, const size
 int b200_poly_div(int field_id, const void* f, size_t n, const void* u, void* out);
 int b200_poly_div_dev(int field_id, const void* f, size_t n, const void* u, void* out, void* stream);
 
+/* ---- Mercury prover pieces (provider/mercury.rs) ---------------------------------------------
+ * f is the coefficient vector of a univariate polynomial read as a row-major rows x cols matrix. */
+/* out[r] = sum_c f[r*cols + c] * v[c], r < rows  (compute_h_poly, mercury.rs:369-386) */
+int b200_mat_vec_rows(int field_id, const void* f, size_t rows, size_t cols, const void* v, void* out);
+int b200_mat_vec_rows_dev(int field_id, const void* f, size_t rows, size_t cols, const void* v, void* out,
+                          void* stream);
+/* f = (X^cols - alpha) q + g  (divide_by_binomial, mercury.rs:319-356): every column c of f, as a polynomial in
+ * Y = X^cols, is divided by (Y - alpha).  q receives (rows-1)*cols coefficients in row-major order, q[r*cols + c]
+ * (the reference's quotient after its transpose; may be NULL when rows == 1), g[c] = column c at alpha.
+ * B200_E_ARG if rows or cols is 0. */
+int b200_div_binomial(int field_id, const void* f, size_t rows, size_t cols, const void* alpha, void* q, void* g);
+int b200_div_binomial_dev(int field_id, const void* f, size_t rows, size_t cols, const void* alpha, void* q,
+                          void* g, void* stream);
+/* the s polynomial of the inner-product step (make_s_polynomial, mercury.rs:391-475), b - 1 coefficients:
+ *   out[k] = sum_j (a1[j+k+1] b1[j] + a1[j] b1[j+k+1]) + gamma * sum_j (a2[j+k+1] b2[j] + a2[j] b2[j+k+1]),
+ * k < b-1, j <= b-k-2; a1, b1, a2, b2 have b entries.  Computed directly (about 2b^2 products), not by NTT. */
+int b200_mercury_s_poly(int field_id, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
+                        const void* gamma, void* out);
+int b200_mercury_s_poly_dev(int field_id, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
+                            const void* gamma, void* out, void* stream);
+
 /* ---- inner-product argument (provider/ipa_pc.rs:174-285), "next" row (f)1 of SURVEY.md §8 ------
  * The reference folds the commitment key every round (ck.fold, pedersen.rs:484-497: n/2 two-point
  * MSMs) and commits over the folded key.  Equivalent and GPU-friendlier: keep the ORIGINAL key

@@ -60,8 +60,11 @@ struct field_ops {
   // evals[q] = f(us[q]), q < nu <= 3, coalesced strided Horner; scratch >= POLY_EVAL_SCRATCH_ELEMS*32 B
   void (*poly_eval)(cudaStream_t, const void* f, size_t n, const void* us, int nu, void* scratch,
                     void* evals);
-  // quotient f / (X - u) (n-1 coefficients); scratch >= poly_div_scratch_elems(n) * 32 B
-  void (*poly_div)(cudaStream_t, const void* f, size_t n, const void* u, void* scratch, void* out);
+  // quotient f / (X - u) (n-1 coefficients) of each of `cols` interleaved polynomials of n coefficients
+  // (coefficient k of column j at f[k * cols + j], quotient likewise in out); rem_or_null receives the
+  // cols remainders f_j(u).  scratch >= poly_div_scratch_elems(n, cols) * 32 B
+  void (*poly_div)(cudaStream_t, const void* f, size_t n, size_t cols, const void* u, void* scratch, void* out,
+                   void* rem_or_null);
   void (*spmv_classify)(cudaStream_t, const void* vals, size_t nnz, int8_t* codes);
   void (*spmv)(cudaStream_t, const uint32_t* indptr, const uint32_t* cols, const int8_t* codes,
                const void* vals, size_t rows, const void* z1, const void* z2_or_null, void* o1,
@@ -111,6 +114,10 @@ struct field_ops {
   // every remaining round of a batched sum-check in one CTA (sumcheck_tail.cuh); sums: 6 * 16 elements of scratch
   void (*scb_tail)(cudaStream_t, const scb_tail_args&, void* state, void* sums, const void* pending,
                    uint32_t pending_len, int absorb_label, int squeeze_label, void* polys, void* rs);
+  // Mercury (mercury.rs): out[r] = sum_c f[r*cols + c] v[c]; the s polynomial (b - 1 coefficients, k_mercury_s_poly)
+  void (*mat_vec_rows)(cudaStream_t, const void* f, size_t rows, size_t cols, const void* v, void* out);
+  void (*mercury_s_poly)(cudaStream_t, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
+                         const void* gamma, void* out);
 };
 // SM count of the H100 SXM (sm_90a): grids below are sized in whole waves of it
 constexpr int NUM_SMS = 132;
@@ -128,10 +135,12 @@ inline bool sc_segmented_enabled() {
 }
 constexpr size_t POLY_EVAL_SCRATCH_ELEMS = (size_t)3 * (1 + SC_MAX_BLOCKS + 256) + (size_t)3 * SC_MAX_BLOCKS;
 constexpr int POLY_CHUNK_HOST = 64;  // must equal POLY_CHUNK in poly_kernels.cuh
-inline size_t poly_div_scratch_elems(size_t n) {
+inline size_t poly_div_scratch_elems(size_t n, size_t cols = 1) {
   size_t t1 = (n + POLY_CHUNK_HOST - 1) / POLY_CHUNK_HOST, t2 = (t1 + POLY_CHUNK_HOST - 1) / POLY_CHUNK_HOST;
-  return 2 * t1 + 2 * t2 + 8;
+  return cols * (2 * t1 + 2 * t2 + 1) + 8;
 }
+// above this many chunks per polynomial the carries are scanned in two levels
+constexpr size_t POLY_DIV_ONE_LEVEL_CHUNKS = 8192;
 
 extern const field_ops OPS_BN254_FR, OPS_BN254_FQ, OPS_PALLAS_FP, OPS_PALLAS_FQ;
 

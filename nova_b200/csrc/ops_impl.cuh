@@ -337,27 +337,47 @@ struct ops_impl {
   // h = f / (X - u).  Level 1: chunk values V1 (Horner per 64 coefficients).  If there are few
   // chunks a single block scans them; otherwise the same two kernels run one level up (V1 as a
   // polynomial in y = u^64) so the single-block scan only ever sees <= ~n/4096 values.
-  static void poly_div(cudaStream_t s, const void* f, size_t n, const void* u, void* scratch, void* out) {
+  //
+  // With cols > 1 the same kernels divide every column of a row-major matrix (divide_by_binomial,
+  // mercury.rs:319-356): one thread per (chunk, column), one scan block per column.  One polynomial keeps
+  // the 512-thread scan block; a column with few chunks gets a block just wide enough for them.
+  static void poly_div(cudaStream_t s, const void* f, size_t n, size_t cols, const void* u, void* scratch, void* out,
+                       void* rem) {
     static_assert(POLY_CHUNK == POLY_CHUNK_HOST, "chunk constants out of sync");
     size_t T1 = (n + POLY_CHUNK - 1) / POLY_CHUNK, T2 = (T1 + POLY_CHUNK - 1) / POLY_CHUNK;
     char* base = (char*)scratch;
     void* v1 = base;
-    void* s1 = base + T1 * 32;
-    void* v2 = base + 2 * T1 * 32;
-    void* s2 = base + (2 * T1 + T2) * 32;
-    void* y = base + (2 * T1 + 2 * T2) * 32;
-    void* ev = base + (2 * T1 + 2 * T2 + 1) * 32;
-    unsigned g1 = (unsigned)((T1 + 127) / 128), g2 = (unsigned)((T2 + 127) / 128);
-    k_poly_chunk_vals<F><<<g1, 128, 0, s>>>(f, n, u, 1, v1);
-    if (T1 <= 8192) {
-      k_poly_suffix<F><<<1, 512, 0, s>>>(v1, T1, u, s1, ev);
+    void* s1 = base + T1 * cols * 32;
+    void* v2 = base + 2 * T1 * cols * 32;
+    void* s2 = base + (2 * T1 + T2) * cols * 32;
+    void* y = base + (2 * T1 + 2 * T2) * cols * 32;
+    void* ev = rem ? rem : base + ((2 * T1 + 2 * T2) * cols + 1) * 32;
+    unsigned g1 = (unsigned)((T1 * cols + 127) / 128), g2 = (unsigned)((T2 * cols + 127) / 128);
+    auto scan_threads = [cols](size_t T) {
+      unsigned nt = 32;
+      while (cols > 1 && nt < 512 && nt < T) nt *= 2;
+      return cols == 1 ? 512u : nt;
+    };
+    k_poly_chunk_vals<F><<<g1, 128, 0, s>>>(f, n, cols, u, 1, v1);
+    if (T1 <= POLY_DIV_ONE_LEVEL_CHUNKS) {
+      k_poly_suffix<F><<<(unsigned)cols, scan_threads(T1), 0, s>>>(v1, T1, cols, u, s1, ev);
     } else {
       k_fe_pow<F><<<1, 32, 0, s>>>(u, POLY_CHUNK, y);
-      k_poly_chunk_vals<F><<<g2, 128, 0, s>>>(v1, T1, y, 1, v2);
-      k_poly_suffix<F><<<1, 512, 0, s>>>(v2, T2, y, s2, ev);
-      k_poly_div_apply<F><<<g2, 128, 0, s>>>(v1, T1, y, s2, T1, s1);  // carries into level-1 chunks
+      k_poly_chunk_vals<F><<<g2, 128, 0, s>>>(v1, T1, cols, y, 1, v2);
+      k_poly_suffix<F><<<(unsigned)cols, scan_threads(T2), 0, s>>>(v2, T2, cols, y, s2, ev);
+      k_poly_div_apply<F><<<g2, 128, 0, s>>>(v1, T1, cols, y, s2, T1, s1);  // carries into level-1 chunks
     }
-    k_poly_div_apply<F><<<g1, 128, 0, s>>>(f, n, u, s1, n - 1, out);
+    k_poly_div_apply<F><<<g1, 128, 0, s>>>(f, n, cols, u, s1, n - 1, out);
+  }
+  static void mat_vec_rows(cudaStream_t s, const void* f, size_t rows, size_t cols, const void* v, void* out) {
+    unsigned grid = (unsigned)(rows < (size_t)NUM_SMS * 64 ? rows : (size_t)NUM_SMS * 64);
+    if (grid) k_mat_vec_rows<F><<<grid, 256, 0, s>>>(f, rows, cols, v, out);
+  }
+  static void mercury_s_poly(cudaStream_t s, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
+                             const void* gamma, void* out) {
+    size_t pairs = b / 2;
+    unsigned grid = (unsigned)(pairs < (size_t)NUM_SMS * 64 ? pairs : (size_t)NUM_SMS * 64);
+    if (grid) k_mercury_s_poly<F><<<grid, 256, 0, s>>>(a1, b1, a2, b2, b, gamma, out);
   }
   static void spmv_classify(cudaStream_t s, const void* vals, size_t nnz, int8_t* codes) {
     k_spmv_classify<F><<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(vals, nnz, codes);
@@ -460,7 +480,7 @@ struct ops_impl {
                      sc_round, fe_inv_each, digits_range, sc_round_batched, on_curve,
                      powers_canonical, scalar_bases, poseidon_ro, to_mont, exchange_identity,
                      sc_round_batched_fused, sc_reduce_multi_partials, gather_heads, poly_eval_small_multi,
-                     eq_prefix_tables, sc_reduce_multi, scb_tail};
+                     eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly};
   }
 };
 

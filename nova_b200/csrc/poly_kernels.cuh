@@ -13,6 +13,8 @@
 //   HyperKZG fold / Horner evaluation / divide by (X-u)      src/provider/hyperkzg.rs:1083-1095,
 //                                                            1011-1019, 961-999
 //   PrecomputedSparseMatrix::multiply_vec(_pair)             src/r1cs/sparse.rs:136-230
+//   Mercury compute_h_poly / divide_by_binomial / make_s_polynomial
+//                                                            src/provider/mercury.rs:369-386, 319-356, 391-475
 #pragma once
 #if !defined(NOVA_SIMT_HOST)  // tests/hostcheck/simt_host.h supplies the few CUDA names the kernels use
 #include <cuda_runtime.h>
@@ -584,34 +586,44 @@ __global__ void __launch_bounds__(256) k_poly_eval_small_multi(poly_multi_args a
 }
 
 constexpr int POLY_CHUNK = 64;
+// The division kernels below take `cols` interleaved polynomials of n coefficients each: coefficient k
+// of column j is b[k * cols + j] (divide_by_binomial, mercury.rs:319-356, divides every column of the
+// row-major matrix f by (Y - alpha)).  cols = 1 is the plain polynomial of hyperkzg.rs:961-999.  Chunk
+// values and carries are laid out [point][chunk][column], so neighbouring threads touch neighbouring
+// columns and every load is coalesced.
+//
 // chunk values V_c = sum_{k<len_c} B[c*m + k] u^k  for each of the NU points (Horner per chunk)
 template <class F>
-__global__ void __launch_bounds__(128) k_poly_chunk_vals(const void* __restrict__ b, size_t n,
+__global__ void __launch_bounds__(128) k_poly_chunk_vals(const void* __restrict__ b, size_t n, size_t cols,
                                                          const void* __restrict__ us, int nu,
-                                                         void* __restrict__ vals /* [nu][T] */) {
+                                                         void* __restrict__ vals /* [nu][T][cols] */) {
   size_t T = (n + POLY_CHUNK - 1) / POLY_CHUNK;
   size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= T) return;
-  size_t lo = t * POLY_CHUNK, hi = lo + POLY_CHUNK < n ? lo + POLY_CHUNK : n;
+  if (t >= T * cols) return;
+  size_t c = t / cols, j = t - c * cols;
+  size_t lo = c * POLY_CHUNK, hi = lo + POLY_CHUNK < n ? lo + POLY_CHUNK : n;
   for (int q = 0; q < nu; q++) {
     fe_t u = fe_load(us, q);
     fe_t acc = fe_zero<F>();
-    for (size_t i = hi; i-- > lo;) acc = fe_add<F>(fe_mul<F>(acc, u), fe_load(b, i));
-    fe_store(vals, (size_t)q * T + t, acc);
+    for (size_t i = hi; i-- > lo;) acc = fe_add<F>(fe_mul<F>(acc, u), fe_load(b, i * cols + j));
+    fe_store(vals, (size_t)q * T * cols + t, acc);
   }
 }
 
-// single block per point: suffix recurrence over chunk values
+// one block per (point, column): suffix recurrence over chunk values
 //   H_c = V_{c+1} + y * H_{c+1},  H_{T-1} = 0,  y = u^m      (carry into chunk c from above)
 // and the polynomial value  P(u) = V_0 + y * H_0.  Affine maps x -> a*x + b are composed with a
-// block-wide scan.  suffix[q][c] = H_c, evals[q] = P(u_q).
+// block-wide scan.  suffix[q][c][j] = H_c, evals[q][j] = P_j(u_q).
 template <class F>
-__global__ void __launch_bounds__(512) k_poly_suffix(const void* __restrict__ vals, size_t T,
+__global__ void __launch_bounds__(512) k_poly_suffix(const void* __restrict__ vals, size_t T, size_t cols,
                                                       const void* __restrict__ us,
                                                       void* __restrict__ suffix,
                                                       void* __restrict__ evals) {
   __shared__ fe_t sa[512], sb[512];
-  const int q = blockIdx.x;
+  const size_t q = blockIdx.x / cols, col = blockIdx.x - q * cols;
+  // chunk c of this (point, column) at element (q * T + c) * cols + col of vals / suffix
+  const void* v = (const char*)vals + 32 * (q * T * cols + col);
+  void* sfx = (char*)suffix + 32 * (q * T * cols + col);
   const fe_t y = fe_pow_u64<F>(fe_load(us, q), POLY_CHUNK);
   const int nt = blockDim.x, tid = threadIdx.x;
   // thread tid owns chunk indices [clo, chi) ; processed from high to low
@@ -625,7 +637,7 @@ __global__ void __launch_bounds__(512) k_poly_suffix(const void* __restrict__ va
   for (size_t c = chi; c-- > clo;) {
     // new = V_c + y * (a*x + b) = (y a) x + (y b + V_c)
     a = fe_mul<F>(y, a);
-    b = fe_add<F>(fe_mul<F>(y, b), fe_load(vals, (size_t)q * T + c));
+    b = fe_add<F>(fe_mul<F>(y, b), fe_load(v, c * cols));
   }
   sa[tid] = a;
   sb[tid] = b;
@@ -650,10 +662,10 @@ __global__ void __launch_bounds__(512) k_poly_suffix(const void* __restrict__ va
   }
   // carry entering the top of my range = total_{tid+1}(0) = sb[tid+1]
   fe_t carry = (tid + 1 < nt) ? sb[tid + 1] : fe_zero<F>();
-  if (tid == 0) fe_store(evals, q, sb[0]);  // total_0(0) = P(u)
+  if (tid == 0) fe_store(evals, blockIdx.x, sb[0]);  // total_0(0) = P(u)
   for (size_t c = chi; c-- > clo;) {
-    fe_store(suffix, (size_t)q * T + c, carry);
-    carry = fe_add<F>(fe_load(vals, (size_t)q * T + c), fe_mul<F>(y, carry));
+    fe_store(sfx, c * cols, carry);
+    carry = fe_add<F>(fe_load(v, c * cols), fe_mul<F>(y, carry));
   }
 }
 
@@ -675,22 +687,72 @@ __global__ void __launch_bounds__(128) k_powers_canonical(const void* __restrict
 
 // quotient by (X - u): h[k-1] = B[k] + u*h[k], h[n-1] := 0  (hyperkzg.rs:961-999); chunk c starts
 // from the carry H_c computed above.  out[k] = h[k] for k < out_len (n-1 for the quotient; n when the
-// same recurrence is reused one level up to spread carries over the level-1 chunks).
+// same recurrence is reused one level up to spread carries over the level-1 chunks).  Per column j of
+// `cols` interleaved polynomials: h_j[k] lands at out[k * cols + j].
 template <class F>
-__global__ void __launch_bounds__(128) k_poly_div_apply(const void* __restrict__ b, size_t n,
+__global__ void __launch_bounds__(128) k_poly_div_apply(const void* __restrict__ b, size_t n, size_t cols,
                                                         const void* __restrict__ u_ptr,
                                                         const void* __restrict__ suffix,
                                                         size_t out_len, void* __restrict__ out) {
   size_t T = (n + POLY_CHUNK - 1) / POLY_CHUNK;
   size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= T) return;
+  if (t >= T * cols) return;
   const fe_t u = fe_load(u_ptr, 0);
-  size_t lo = t * POLY_CHUNK, hi = lo + POLY_CHUNK < n ? lo + POLY_CHUNK : n;
+  size_t c = t / cols, j = t - c * cols;
+  size_t lo = c * POLY_CHUNK, hi = lo + POLY_CHUNK < n ? lo + POLY_CHUNK : n;
   fe_t carry = fe_load(suffix, t);  // = h[hi-1]
   for (size_t k = hi; k-- > lo;) {
     // carry == h[k];  h[k-1] = B[k] + u*h[k]
-    if (k < out_len) fe_store(out, k, carry);
-    carry = fe_add<F>(fe_load(b, k), fe_mul<F>(u, carry));
+    if (k < out_len) fe_store(out, k * cols + j, carry);
+    carry = fe_add<F>(fe_load(b, k * cols + j), fe_mul<F>(u, carry));
+  }
+}
+
+// ------------------------------------------------------------------------------------------
+// Mercury prover pieces (provider/mercury.rs)
+// ------------------------------------------------------------------------------------------
+// compute_h_poly (mercury.rs:369-386): out[r] = sum_c f[r*cols + c] * v[c].  One block per row (grid-
+// stride over rows), threads stride over the columns: coalesced reads of f, v stays in L2.
+template <class F>
+__global__ void __launch_bounds__(256) k_mat_vec_rows(const void* __restrict__ f, size_t rows, size_t cols,
+                                                      const void* __restrict__ v, void* __restrict__ out) {
+  __shared__ fe_t sm[8];
+  for (size_t r = blockIdx.x; r < rows; r += gridDim.x) {
+    fe_t acc[1] = {fe_zero<F>()};
+    const void* row = (const char*)f + 32 * r * cols;
+    for (size_t c = threadIdx.x; c < cols; c += blockDim.x)
+      acc[0] = fe_add<F>(acc[0], fe_mul<F>(fe_load(row, c), fe_load(v, c)));
+    block_sum<F, 1>(acc, sm);
+    if (threadIdx.x == 0) fe_store(out, r, acc[0]);
+    __syncthreads();  // sm is reused by the next row
+  }
+}
+
+// make_s_polynomial (mercury.rs:391-475) without an NTT: s[k] is the coefficient of X^(k+1) (lag m = k+1)
+// of a1(X) b1(1/X) + a1(1/X) b1(X) + gamma (a2(X) b2(1/X) + a2(1/X) b2(X)):
+//   s[m-1] = sum_{j <= b-1-m} (a1[j+m] b1[j] + a1[j] b1[j+m]) + gamma * (the same over a2, b2),  1 <= m < b.
+// Lag m has b - m terms, so block i takes the lags i+1 and b-1-i (b terms together, one lag when they meet).
+template <class F>
+__global__ void __launch_bounds__(256) k_mercury_s_poly(const void* __restrict__ a1, const void* __restrict__ b1,
+                                                        const void* __restrict__ a2, const void* __restrict__ b2,
+                                                        size_t b, const void* __restrict__ gamma_ptr,
+                                                        void* __restrict__ out) {
+  __shared__ fe_t sm[8 * 2];
+  for (size_t i = blockIdx.x; i < b / 2; i += gridDim.x) {
+    const int nl = i + 1 == b - 1 - i ? 1 : 2;
+    for (int l = 0; l < nl; l++) {
+      const size_t m = l == 0 ? i + 1 : b - 1 - i;
+      fe_t acc[2] = {fe_zero<F>(), fe_zero<F>()};
+      for (size_t j = threadIdx.x; j + m < b; j += blockDim.x) {
+        acc[0] = fe_add<F>(acc[0], fe_add<F>(fe_mul<F>(fe_load(a1, j + m), fe_load(b1, j)),
+                                             fe_mul<F>(fe_load(a1, j), fe_load(b1, j + m))));
+        acc[1] = fe_add<F>(acc[1], fe_add<F>(fe_mul<F>(fe_load(a2, j + m), fe_load(b2, j)),
+                                             fe_mul<F>(fe_load(a2, j), fe_load(b2, j + m))));
+      }
+      block_sum<F, 2>(acc, sm);
+      if (threadIdx.x == 0) fe_store(out, m - 1, fe_add<F>(acc[0], fe_mul<F>(fe_load(gamma_ptr, 0), acc[1])));
+      __syncthreads();
+    }
   }
 }
 

@@ -120,6 +120,12 @@ SIGNATURES = {
     "b200_poly_eval_many_dev": [c_int, _P, _P, c_size_t, _P, c_size_t, _P, _P],
     "b200_poly_div": [c_int, _P, c_size_t, _P, _P],
     "b200_poly_div_dev": [c_int, _P, c_size_t, _P, _P, _P],
+    "b200_mat_vec_rows": [c_int, _P, c_size_t, c_size_t, _P, _P],
+    "b200_mat_vec_rows_dev": [c_int, _P, c_size_t, c_size_t, _P, _P, _P],
+    "b200_div_binomial": [c_int, _P, c_size_t, c_size_t, _P, _P, _P],
+    "b200_div_binomial_dev": [c_int, _P, c_size_t, c_size_t, _P, _P, _P, _P],
+    "b200_mercury_s_poly": [c_int, _P, _P, _P, _P, c_size_t, _P, _P],
+    "b200_mercury_s_poly_dev": [c_int, _P, _P, _P, _P, c_size_t, _P, _P, _P],
     "b200_spmv_register": [c_int, _P, ctypes.POINTER(c_u64), ctypes.POINTER(c_u64), c_size_t, c_size_t,
                            ctypes.POINTER(c_u64)],
     "b200_spmv_release": [c_u64],

@@ -924,14 +924,39 @@ def prove_core(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: 
 
 
 def prove(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: dict, vk_digest: int, transcript,
-          timings: dict | None = None, device_transcript: bool = False):
-    """The whole RelaxedR1CSSNARK::prove of ppsnark.rs:1056-1385: prove_core, then EE::prove (HyperKZG with the
-    transcript) on the batched polynomial at r_inner_batched.  (The batched commitment sum_i c^i C_i of
-    PolyEvalInstance::batch is only an input of EE::prove for the transcript-free HyperKZG prover, which does
-    not use it: the caller / verifier forms it from the 15 commitments.)  -> proof fields + `eval_arg`."""
-    from .spartan import hyperkzg_prove
+          timings: dict | None = None, device_transcript: bool = False, ee: str = "hyperkzg",
+          S_comm: dict | None = None):
+    """The whole RelaxedR1CSSNARK::prove of ppsnark.rs:1056-1385: prove_core, then EE::prove with the transcript
+    on the batched polynomial at r_inner_batched.  -> proof fields + `eval_arg`.
+      ee = "hyperkzg": hyperkzg.rs:926-1116.  (The batched commitment sum_i c^i C_i of PolyEvalInstance::batch
+                       is only an input of EE::prove for the HyperKZG prover, which does not use it: the caller /
+                       verifier forms it from the 15 commitments.)
+      ee = "mercury":  mercury.rs:891-1268, which absorbs the batched commitment: `S_comm` must hold the seven
+                       shape commitments (R1CSShapeSparkCommitment: val_A, val_B, val_C, row, col, ts_row, ts_col)."""
+    if ee not in ("hyperkzg", "mercury"):
+        raise ValueError(f"unknown evaluation engine {ee!r}")
+    if ee == "mercury" and S_comm is None:
+        raise ValueError("the Mercury evaluation argument needs the shape commitments S_comm")
     out = prove_core(curve, ck, S, spark, U, W, vk_digest, transcript, timings, device_transcript)
-    out["eval_arg"] = hyperkzg_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings)
+    if ee == "hyperkzg":
+        from .spartan import hyperkzg_prove
+        out["eval_arg"] = hyperkzg_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings)
+        return out
+    from .mercury import mercury_prove
+    from .provider import Curve, DlogGroup
+    from .snark import _affine_bytes
+    curve = Curve(curve)
+    fid = curve.scalar_field
+    p = fields.MODULUS[fid]
+    cm = out["comm_mem"]
+    comm_vec = [U["comm_W"], U["comm_E"], out["comm_L_row"], out["comm_L_col"], S_comm["val_A"], S_comm["val_B"],
+                S_comm["val_C"], cm[0], S_comm["row"], cm[1], S_comm["ts_row"], cm[2], S_comm["col"], cm[3],
+                S_comm["ts_col"]]  # ppsnark.rs comm_vec order
+    c = out["batch_challenge"]
+    C = DlogGroup(curve).vartime_multiscalar_mul(fields.pack(fid, [pow(c, i, p) for i in range(len(comm_vec))]),
+                                                 b"".join(_affine_bytes(curve, P) for P in comm_vec))
+    out["eval_arg"] = mercury_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings,
+                                    comm=C, eval_=out["batched_eval"])
     return out
 
 

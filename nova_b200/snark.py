@@ -170,11 +170,17 @@ def prove(curve, ck: CommitmentKey, S: dict, U: dict, W: dict, vk_digest: int, t
     the same transcript; `ck` must be the key the commitments in U were made with.
       ee = "hyperkzg": hyperkzg.rs:926-1116 (primary curve, S1)       -> eval_arg = (com, w, v)
       ee = "ipa":      ipa_pc.rs:64-77, 174-285 (secondary curve, S2) -> eval_arg = (L_vec, R_vec, a_hat);
-                       `ck` must carry the generator ck_c as its blinding base."""
+                       `ck` must carry the generator ck_c as its blinding base.
+      ee = "mercury":  mercury.rs:891-1268 (BN254, HyperKZG key)      -> eval_arg = mercury.EvaluationArgument,
+                       on the batched claim (batched_c, batched_x, batched_e)."""
     proof = prove_core(curve, ck, S, U, W, vk_digest, transcript, device_transcript, timings)
     if ee == "hyperkzg":
         from .spartan import hyperkzg_prove
         proof["eval_arg"] = hyperkzg_prove(curve, ck, proof["batched_poly"], proof["batched_x"], transcript, timings)
+    elif ee == "mercury":
+        from .mercury import mercury_prove
+        proof["eval_arg"] = mercury_prove(curve, ck, proof["batched_poly"], proof["batched_x"], transcript, timings,
+                                          comm=proof["batched_c"], eval_=proof["batched_e"])
     elif ee == "ipa":
         from .ipa import InnerProductArgument
         fid = Curve(curve).scalar_field
