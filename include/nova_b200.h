@@ -469,6 +469,29 @@ int b200_mercury_s_poly(int field_id, const void* a1, const void* b1, const void
 int b200_mercury_s_poly_dev(int field_id, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
                             const void* gamma, void* out, void* stream);
 
+/* ---- NeutronNova folding prover pieces (neutron/nifs.rs, neutron/relation.rs) ------------------
+ * A structure of n = left * right rows; row k = i * left + j.  e1, e2 hold left + right entries (the split
+ * power polynomial: e = the first `left`, f = the last `right`); az*, bz*, cz* hold n entries. */
+/* the five sums of NIFS::prove_helper (nifs.rs:29-186) BEFORE its rho factors: with V_t = V1 + t (V2 - V1),
+ *   out[m] = sum_i f_t[i] * sum_j e_t[j] * (Az_t[k] Bz_t[k] - Cz_t[k]),   t = 0, 2, 3, 4, 5 for m = 0..4,
+ * as Montgomery elements.  One pass over the six n-vectors; with the second instance equal to the first every
+ * sum is the is_sat sum (relation.rs:71-116).  B200_E_ARG if left or right is 0. */
+int b200_neutron_evals(int field_id, const void* e1, const void* az1, const void* bz1, const void* cz1,
+                       const void* e2, const void* az2, const void* bz2, const void* cz2, size_t left, size_t right,
+                       void* out);
+int b200_neutron_evals_dev(int field_id, const void* e1, const void* az1, const void* bz1, const void* cz1,
+                           const void* e2, const void* az2, const void* bz2, const void* cz2, size_t left,
+                           size_t right, void* out, void* stream);
+/* PowPolynomial::split_evals (spartan/polys/power.rs:62-86), left + right entries: out[j] = tau^j (j < left),
+ * out[left + i] = tau^(left * i) (i < right).  tau: one element (a device pointer on the _dev form).
+ * B200_E_ARG if left is 0 or right < 2 (the reference indexes right[1]). */
+int b200_pow_split_evals(int field_id, const void* tau, size_t left, size_t right, void* out);
+int b200_pow_split_evals_dev(int field_id, const void* tau, size_t left, size_t right, void* out, void* stream);
+/* out[i] = a[i] + r * (b[i] - a[i]), i < n: the witness folds W1 + r_b (W2 - W1), E1 + r_b (E - E1)
+ * (FoldedWitness::fold, relation.rs:131-156).  out may alias a. */
+int b200_lerp(int field_id, const void* a, const void* b, const void* r, size_t n, void* out);
+int b200_lerp_dev(int field_id, const void* a, const void* b, const void* r, size_t n, void* out, void* stream);
+
 /* ---- inner-product argument (provider/ipa_pc.rs:174-285), "next" row (f)1 of SURVEY.md §8 ------
  * The reference folds the commitment key every round (ck.fold, pedersen.rs:484-497: n/2 two-point
  * MSMs) and commits over the folded key.  Equivalent and GPU-friendlier: keep the ORIGINAL key

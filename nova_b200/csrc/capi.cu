@@ -1892,3 +1892,4 @@ int b200_bind_top(int fid, void* z, size_t n, const void* r) {
 #include "capi_poly.inc"
 #include "capi_sumcheck.inc"
 #include "capi_stream.inc"
+#include "capi_neutron.inc"

@@ -4,6 +4,7 @@
 //
 //   k_cross_term  T = Az o Bz - u*Cz - E1 (- E2)      src/r1cs/mod.rs:614-620, 650-657
 //   k_axpy        out = a + r*b                        src/r1cs/mod.rs:1044-1073 (W, E folds)
+//   k_lerp        out = a + r*(b - a)                  src/neutron/relation.rs:139-153 (W, E folds)
 //   k_vec_add     out = a + b                          src/r1cs/mod.rs:589-609 (Z = Z1 + Z2)
 //   k_bind_top    Z[i] += r*(Z[i+n/2] - Z[i])          src/spartan/polys/multilinear.rs:65-84
 //   k_vec_mul     out = a o b                          src/spartan/ppsnark.rs:446-449 (inv o TS)
@@ -42,6 +43,19 @@ __global__ void __launch_bounds__(256) k_axpy(const void* __restrict__ a,
        i += (size_t)gridDim.x * blockDim.x) {
     fe_t x = fe_load(a, i), y = fe_load(b, i);
     fe_store(out, i, fe_add<F>(x, fe_mul<F>(r, y)));
+  }
+}
+
+// out = a + r*(b - a).  out may alias a: each element is read and then written by one thread, and `a`
+// goes through the coherent load path because the kernel writes that buffer.
+template <class F>
+__global__ void __launch_bounds__(256) k_lerp(const void* a, const void* __restrict__ b,
+                                              const void* __restrict__ r_ptr, size_t n, void* out) {
+  const fe_t r = fe_load(r_ptr, 0);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n;
+       i += (size_t)gridDim.x * blockDim.x) {
+    fe_t x = fe_load_rw(a, i), y = fe_load(b, i);
+    fe_store(out, i, fe_add<F>(x, fe_mul<F>(r, fe_sub<F>(y, x))));
   }
 }
 

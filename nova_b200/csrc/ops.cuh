@@ -118,6 +118,13 @@ struct field_ops {
   void (*mat_vec_rows)(cudaStream_t, const void* f, size_t rows, size_t cols, const void* v, void* out);
   void (*mercury_s_poly)(cudaStream_t, const void* a1, const void* b1, const void* a2, const void* b2, size_t b,
                          const void* gamma, void* out);
+  // NeutronNova (neutron/nifs.rs, relation.rs): the five raw sums of prove_helper (k_neutron_evals; scratch >=
+  // neutron_evals_scratch_elems(left * right) * 32 B), split_evals of the power polynomial, out = a + r (b - a)
+  void (*neutron_evals)(cudaStream_t, const void* e1, const void* az1, const void* bz1, const void* cz1,
+                        const void* e2, const void* az2, const void* bz2, const void* cz2, size_t left, size_t right,
+                        void* scratch, void* out);
+  void (*pow_split_evals)(cudaStream_t, const void* tau, size_t left, size_t right, void* out);
+  void (*lerp)(cudaStream_t, const void* a, const void* b, const void* r, size_t n, void* out);
 };
 // SM count of the H100 SXM (sm_90a): grids below are sized in whole waves of it
 constexpr int NUM_SMS = 132;
@@ -141,6 +148,14 @@ inline size_t poly_div_scratch_elems(size_t n, size_t cols = 1) {
 }
 // above this many chunks per polynomial the carries are scanned in two levels
 constexpr size_t POLY_DIV_ONE_LEVEL_CHUNKS = 8192;
+// k_neutron_evals: one block per tile of at least NEUTRON_ROWS_PER_BLOCK rows, at most NEUTRON_MAX_BLOCKS blocks
+constexpr size_t NEUTRON_ROWS_PER_BLOCK = 1024;
+constexpr size_t NEUTRON_MAX_BLOCKS = (size_t)NUM_SMS * 8;
+inline size_t neutron_evals_blocks(size_t n) {
+  size_t g = (n + NEUTRON_ROWS_PER_BLOCK - 1) / NEUTRON_ROWS_PER_BLOCK;
+  return g < 1 ? 1 : (g > NEUTRON_MAX_BLOCKS ? NEUTRON_MAX_BLOCKS : g);
+}
+inline size_t neutron_evals_scratch_elems(size_t n) { return 5 * neutron_evals_blocks(n); }
 
 extern const field_ops OPS_BN254_FR, OPS_BN254_FQ, OPS_PALLAS_FP, OPS_PALLAS_FQ;
 

@@ -379,6 +379,20 @@ struct ops_impl {
     unsigned grid = (unsigned)(pairs < (size_t)NUM_SMS * 64 ? pairs : (size_t)NUM_SMS * 64);
     if (grid) k_mercury_s_poly<F><<<grid, 256, 0, s>>>(a1, b1, a2, b2, b, gamma, out);
   }
+  static void neutron_evals(cudaStream_t s, const void* e1, const void* az1, const void* bz1, const void* cz1,
+                            const void* e2, const void* az2, const void* bz2, const void* cz2, size_t left,
+                            size_t right, void* scratch, void* out) {
+    const size_t n = left * right, grid = neutron_evals_blocks(n), tile = (n + grid - 1) / grid;
+    k_neutron_evals<F><<<(unsigned)grid, 256, 0, s>>>(e1, az1, bz1, cz1, e2, az2, bz2, cz2, left, right, tile,
+                                                      scratch);
+    k_form_final<F, 5><<<1, 256, 0, s>>>(scratch, (int)grid, out);
+  }
+  static void pow_split_evals(cudaStream_t s, const void* tau, size_t left, size_t right, void* out) {
+    k_pow_split_evals<F><<<stream_grid(left + right, 128), 128, 0, s>>>(tau, left, right, out);
+  }
+  static void lerp(cudaStream_t s, const void* a, const void* b, const void* r, size_t n, void* out) {
+    k_lerp<F><<<stream_grid(n, 256), 256, 0, s>>>(a, b, r, n, out);
+  }
   static void spmv_classify(cudaStream_t s, const void* vals, size_t nnz, int8_t* codes) {
     k_spmv_classify<F><<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(vals, nnz, codes);
   }
@@ -480,7 +494,8 @@ struct ops_impl {
                      sc_round, fe_inv_each, digits_range, sc_round_batched, on_curve,
                      powers_canonical, scalar_bases, poseidon_ro, to_mont, exchange_identity,
                      sc_round_batched_fused, sc_reduce_multi_partials, gather_heads, poly_eval_small_multi,
-                     eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly};
+                     eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly,
+                     neutron_evals, pow_split_evals, lerp};
   }
 };
 

@@ -860,4 +860,85 @@ static __global__ void __launch_bounds__(256) k_gather32(const void* __restrict_
     fe_store(out, i, fe_load(table, idx[i]));
 }
 
+// ------------------------------------------------------------------------------------------
+// NeutronNova folding prover pieces (neutron/nifs.rs, spartan/polys/power.rs)
+// ------------------------------------------------------------------------------------------
+// prove_helper (nifs.rs:29-186) before the rho factors.  Row k = i*left + j; with V_t = V1 + t (V2 - V1)
+// for e (first `left` entries of e1/e2), f (the `right` entries after them), Az, Bz, Cz:
+//   S_t = sum_i f_t[i] * sum_j e_t[j] (Az_t[k] Bz_t[k] - Cz_t[k]),   t in {0, 2, 3, 4, 5}.
+// Each block owns a contiguous tile of rows and its threads stride through it by blockDim, so loads
+// stay coalesced and a thread meets the same i for about left / blockDim rows in a row: the inner sums
+// are kept per thread and multiplied by f_t[i] only when i changes (10 products per row plus 5 per
+// change).  partials[block][t] feed k_form_final<F, 5>; field sums are exact, so the tiling does not
+// change the result.
+template <class F>
+__global__ void __launch_bounds__(256) k_neutron_evals(const void* __restrict__ e1, const void* __restrict__ az1,
+                                                       const void* __restrict__ bz1, const void* __restrict__ cz1,
+                                                       const void* __restrict__ e2, const void* __restrict__ az2,
+                                                       const void* __restrict__ bz2, const void* __restrict__ cz2,
+                                                       size_t left, size_t right, size_t tile,
+                                                       void* __restrict__ partials) {
+  __shared__ fe_t sm[8 * 5];
+  const size_t n = left * right;
+  const size_t lo = (size_t)blockIdx.x * tile, hi = lo + tile < n ? lo + tile : n;
+  fe_t acc[5], inner[5];
+#pragma unroll
+  for (int t = 0; t < 5; t++) acc[t] = inner[t] = fe_zero<F>();
+  const void* f1 = (const char*)e1 + 32 * left;
+  const void* f2 = (const char*)e2 + 32 * left;
+  // inner[] -> acc[]: acc_t += f_t[i] * inner_t
+  auto flush = [&](size_t i) {
+    fe_t fv = fe_load(f1, i), fh = fe_load(f2, i), d = fe_sub<F>(fh, fv);
+    acc[0] = fe_add<F>(acc[0], fe_mul<F>(fv, inner[0]));
+    fv = fe_add<F>(fh, d);  // t = 2
+#pragma unroll
+    for (int t = 1; t < 5; t++) {
+      acc[t] = fe_add<F>(acc[t], fe_mul<F>(fv, inner[t]));
+      fv = fe_add<F>(fv, d);
+    }
+  };
+  size_t cur = ~(size_t)0;
+  for (size_t k = lo + threadIdx.x; k < hi; k += blockDim.x) {
+    const size_t i = k / left, j = k - i * left;
+    if (i != cur) {
+      if (cur != ~(size_t)0) flush(cur);
+#pragma unroll
+      for (int t = 0; t < 5; t++) inner[t] = fe_zero<F>();
+      cur = i;
+    }
+    fe_t e = fe_load(e1, j), a = fe_load(az1, k), b = fe_load(bz1, k), c = fe_load(cz1, k);
+    const fe_t eh = fe_load(e2, j), ah = fe_load(az2, k), bh = fe_load(bz2, k), ch = fe_load(cz2, k);
+    const fe_t de = fe_sub<F>(eh, e), da = fe_sub<F>(ah, a), db = fe_sub<F>(bh, b), dc = fe_sub<F>(ch, c);
+    inner[0] = fe_add<F>(inner[0], fe_mul<F>(e, fe_sub<F>(fe_mul<F>(a, b), c)));
+    // t = 2: 2 V2 - V1 = V2 + d; then one more d per step
+    e = fe_add<F>(eh, de);
+    a = fe_add<F>(ah, da);
+    b = fe_add<F>(bh, db);
+    c = fe_add<F>(ch, dc);
+#pragma unroll
+    for (int t = 1; t < 5; t++) {
+      inner[t] = fe_add<F>(inner[t], fe_mul<F>(e, fe_sub<F>(fe_mul<F>(a, b), c)));
+      e = fe_add<F>(e, de);
+      a = fe_add<F>(a, da);
+      b = fe_add<F>(b, db);
+      c = fe_add<F>(c, dc);
+    }
+  }
+  if (cur != ~(size_t)0) flush(cur);
+  block_sum<F, 5>(acc, sm);
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int t = 0; t < 5; t++) fe_store(partials, (size_t)blockIdx.x * 5 + t, acc[t]);
+}
+
+// PowPolynomial::split_evals (power.rs:62-86): out[j] = tau^j (j < left), out[left + i] = tau^(left i) (i < right).
+template <class F>
+__global__ void __launch_bounds__(128) k_pow_split_evals(const void* __restrict__ tau_ptr, size_t left, size_t right,
+                                                         void* __restrict__ out) {
+  const fe_t tau = fe_load(tau_ptr, 0);
+  for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < left + right;
+       x += (size_t)gridDim.x * blockDim.x)
+    fe_store(out, x, fe_pow_u64<F>(tau, (uint64_t)(x < left ? x : left * (x - left))));
+}
+
 }  // namespace nova

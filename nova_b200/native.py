@@ -126,6 +126,12 @@ SIGNATURES = {
     "b200_div_binomial_dev": [c_int, _P, c_size_t, c_size_t, _P, _P, _P, _P],
     "b200_mercury_s_poly": [c_int, _P, _P, _P, _P, c_size_t, _P, _P],
     "b200_mercury_s_poly_dev": [c_int, _P, _P, _P, _P, c_size_t, _P, _P, _P],
+    "b200_neutron_evals": [c_int] + [_P] * 8 + [c_size_t, c_size_t, _P],
+    "b200_neutron_evals_dev": [c_int] + [_P] * 8 + [c_size_t, c_size_t, _P, _P],
+    "b200_pow_split_evals": [c_int, _P, c_size_t, c_size_t, _P],
+    "b200_pow_split_evals_dev": [c_int, _P, c_size_t, c_size_t, _P, _P],
+    "b200_lerp": [c_int, _P, _P, _P, c_size_t, _P],
+    "b200_lerp_dev": [c_int, _P, _P, _P, c_size_t, _P, _P],
     "b200_spmv_register": [c_int, _P, ctypes.POINTER(c_u64), ctypes.POINTER(c_u64), c_size_t, c_size_t,
                            ctypes.POINTER(c_u64)],
     "b200_spmv_release": [c_u64],

@@ -222,6 +222,23 @@ class UniPoly:
         b = ((abcd + m1) * pow(2, -1, p) - d) % p
         return cls(p, [d, abcd - a - d - b, b, a])
 
+    @classmethod
+    def from_evals(cls, p, ev):
+        """UniPoly::from_evals (univariate.rs:58-85): the polynomial of degree < len(ev) through (x, ev[x]),
+        x = 0, 1, ...  The reference solves the Vandermonde system by Gaussian elimination; the interpolant is
+        unique, so Lagrange's formula gives the same coefficients."""
+        n = len(ev)
+        coeffs = [0] * n
+        for i, y in enumerate(ev):
+            num, den = [1], 1  # prod_{m != i} (X - m) / (i - m), coefficients lowest first
+            for m in range(n):
+                if m != i:
+                    num = [(a - m * b) % p for a, b in zip([0] + num, num + [0])]
+                    den = den * (i - m) % p
+            k = y * pow(den, -1, p) % p
+            coeffs = [(c + k * a) % p for c, a in zip(coeffs, num)]
+        return cls(p, coeffs)
+
     def evaluate(self, r):
         acc, pw = self.coeffs[0], r
         for c in self.coeffs[1:]:
