@@ -2,6 +2,7 @@
 // Template-free: all kernels are reached through the per-field launcher tables (ops.cuh).
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -77,8 +78,8 @@ int ensure_init() {
   CU(cudaSetDevice(g_dev.device));
   CU(cudaStreamCreateWithFlags(&g_dev.stream, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&g_dev.aux, cudaStreamNonBlocking));
-  // b200_dev_alloc / b200_dev_free and the library's own temporaries come from the device's stream-ordered pool
-  // (cudaMallocAsync on the library stream): a prover allocates and drops dozens of vectors per proof, and
+  // b200_dev_alloc / b200_dev_free and the library's own temporaries (dev_buf) come from the device's stream-ordered
+  // pool (cudaMallocAsync on the library stream, or on the stream a temporary is used on): a prover allocates and drops dozens of vectors per proof, and
   // cudaMalloc / cudaFree cost milliseconds each and synchronise the device (for HyperKZG 2^22 the pool is worth
   // an order of magnitude per proof).  The pool keeps what it has been given (release threshold = max).  NOVA_B200_POOL=0
   // restores plain cudaMalloc / cudaFree.
@@ -98,10 +99,28 @@ int ensure_init() {
   return B200_OK;
 }
 
-cudaError_t pool_alloc(void** p, size_t bytes) {
-  return g_dev.pool ? cudaMallocAsync(p, bytes ? bytes : 1, g_dev.stream) : cudaMalloc(p, bytes ? bytes : 1);
+inline cudaStream_t pick_stream(void* stream) { return stream ? (cudaStream_t)stream : g_dev.stream; }
+
+cudaError_t pool_alloc(void** p, size_t bytes, cudaStream_t s) {
+  return g_dev.pool ? cudaMallocAsync(p, bytes ? bytes : 1, s) : cudaMalloc(p, bytes ? bytes : 1);
 }
-cudaError_t pool_free(void* p) { return g_dev.pool ? cudaFreeAsync(p, g_dev.stream) : cudaFree(p); }
+cudaError_t pool_free(void* p, cudaStream_t s) { return g_dev.pool ? cudaFreeAsync(p, s) : cudaFree(p); }
+
+// Scratch owned by one call, allocated and freed in the order of the stream `s` that uses it (pool_alloc).
+struct dev_buf {
+  void* p = nullptr;
+  cudaStream_t s;
+  explicit dev_buf(cudaStream_t st) : s(st) {}
+  dev_buf(const dev_buf&) = delete;
+  dev_buf& operator=(const dev_buf&) = delete;
+  ~dev_buf() {
+    if (p) pool_free(p, s);
+  }
+  int alloc(size_t bytes) {
+    CU(pool_alloc(&p, bytes, s));
+    return B200_OK;
+  }
+};
 
 // ---------------------------------------------------------------------------------------------
 // commitment-key context
@@ -466,13 +485,6 @@ int enqueue_msm(ck_ctx& ck, size_t base_offset, const void* d_scalars, size_t n,
   return enqueue_msm(ck, ck.ws, base_offset, d_scalars, n, d_out, s, small_elem_bytes, blinded);
 }
 
-struct dev_flag {
-  uint32_t* p = nullptr;
-  ~dev_flag() {
-    if (p) cudaFree(p);
-  }
-};
-
 constexpr size_t SMALL_KEY_MAX = (size_t)1 << 21;
 constexpr int SMALL_KEY_WINDOW = 17;
 
@@ -537,11 +549,11 @@ int register_key(int curve_id, const void* bases, bool bases_on_device, size_t n
     CU(cudaMemcpyAsync((char*)ck->tables + n * 64, h, 64, cudaMemcpyHostToDevice, st));
   if (first_bad) {
     *first_bad = SIZE_MAX;
-    dev_flag flag;
-    CU(cudaMalloc(&flag.p, 4));
+    dev_buf flag(st);
+    if (int rc = flag.alloc(4)) return rc;
     CU(cudaMemsetAsync(flag.p, 0xFF, 4, st));
     ops_for_field(CURVES[curve_id].base_fid)
-        ->on_curve(st, ck->tables, ck->stride, CURVE_B_SMALL[curve_id], flag.p);
+        ->on_curve(st, ck->tables, ck->stride, CURVE_B_SMALL[curve_id], (uint32_t*)flag.p);
     count_launch(1);
     CU(cudaGetLastError());
     uint32_t bad = 0;
@@ -584,17 +596,52 @@ int with_field(int field_id, Fn fn) {
   return fn(ops);
 }
 
-// host-pointer wrapper for the streaming field kernels: stage through device scratch
-struct dev_buf {
-  void* p = nullptr;
-  ~dev_buf() {
-    if (p) pool_free(p);
-  }
-  int alloc(size_t bytes) {
-    CU(pool_alloc(&p, bytes));
-    return B200_OK;
-  }
+inline size_t pad256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// One device region of a host-pointer call: `src` is uploaded into it before the device form runs, and `dst` is
+// downloaded from it afterwards.  The region holds at least `bytes`, `src_bytes` and `dst_bytes`.
+struct host_piece {
+  const void* src;
+  size_t src_bytes;
+  void* dst;
+  size_t dst_bytes;
+  size_t bytes;
 };
+inline host_piece up(const void* src, size_t bytes) { return {src, bytes, nullptr, 0, 0}; }
+inline host_piece down(void* dst, size_t bytes, size_t region = 0) { return {nullptr, 0, dst, bytes, region}; }
+
+// The host-pointer form of a device entry: one pool block on the library stream, one 256-byte aligned region per
+// piece, the uploads, dev(d, s) with d[i] the region of piece i, the downloads, one synchronisation.  A piece without
+// a host pointer gives dev a null pointer, so dev's own checks decide the status; any other piece gets a region, even
+// for 0 bytes.  When dev fails its status is returned and nothing is downloaded.
+template <class Fn>
+int via_device(const std::vector<host_piece>& pieces, Fn dev) {
+  auto region = [](const host_piece& p) {
+    return pad256(std::max({p.src_bytes, p.dst_bytes, p.bytes, (size_t)1}));
+  };
+  size_t total = 0;
+  for (const host_piece& p : pieces)
+    if (p.src || p.dst) total += region(p);
+  const cudaStream_t s = g_dev.stream;
+  dev_buf buf(s);
+  int rc = buf.alloc(total);
+  if (rc) return rc;
+  std::vector<void*> d(pieces.size(), nullptr);
+  char* next = (char*)buf.p;
+  for (size_t i = 0; i < pieces.size(); i++) {
+    const host_piece& p = pieces[i];
+    if (!p.src && !p.dst) continue;
+    d[i] = next;
+    next += region(p);
+    if (p.src && p.src_bytes) CU(cudaMemcpyAsync(d[i], p.src, p.src_bytes, cudaMemcpyHostToDevice, s));
+  }
+  if ((rc = dev(d.data(), s))) return rc;
+  for (size_t i = 0; i < pieces.size(); i++)
+    if (pieces[i].dst && pieces[i].dst_bytes)
+      CU(cudaMemcpyAsync(pieces[i].dst, d[i], pieces[i].dst_bytes, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  return B200_OK;
+}
 
 }  // namespace
 
@@ -635,14 +682,14 @@ int b200_host_free(void* ptr) {
 int b200_dev_alloc(size_t bytes, void** dptr) {
   int rc = ensure_init();
   if (rc) return rc;
-  CU(pool_alloc(dptr, bytes));
+  CU(pool_alloc(dptr, bytes, g_dev.stream));
   return B200_OK;
 }
 int b200_dev_free(void* dptr) {
   if (!dptr) return B200_OK;
   int rc = ensure_init();
   if (rc) return rc;
-  CU(pool_free(dptr));
+  CU(pool_free(dptr, g_dev.stream));
   return B200_OK;
 }
 int b200_memcpy_h2d(void* dptr, const void* hptr, size_t bytes) {
@@ -664,8 +711,7 @@ int b200_memcpy_d2d(void* dst, const void* src, size_t bytes, void* stream) {
   if (rc) return rc;
   if (bytes == 0) return B200_OK;
   if (!dst || !src) return fail(B200_E_ARG, "null pointer");
-  CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice,
-                     stream ? (cudaStream_t)stream : g_dev.stream));
+  CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, pick_stream(stream)));
   return B200_OK;
 }
 int b200_memset_dev(void* dptr, int byte, size_t bytes, void* stream) {
@@ -673,7 +719,7 @@ int b200_memset_dev(void* dptr, int byte, size_t bytes, void* stream) {
   if (rc) return rc;
   if (bytes == 0) return B200_OK;
   if (!dptr) return fail(B200_E_ARG, "null pointer");
-  CU(cudaMemsetAsync(dptr, byte, bytes, stream ? (cudaStream_t)stream : g_dev.stream));
+  CU(cudaMemsetAsync(dptr, byte, bytes, pick_stream(stream)));
   return B200_OK;
 }
 int b200_sync(void) {
@@ -713,7 +759,7 @@ int b200_jacobian_sum_dev(int curve_id, const void* d_points, size_t k, void* d_
   if (curve_id < 0 || curve_id > 3) return fail(B200_E_ARG, "unknown curve id %d", curve_id);
   if (!d_out || (k && !d_points)) return fail(B200_E_ARG, "null pointer");
   const field_ops* bops = ops_for_field(CURVES[curve_id].base_fid);
-  bops->jacobian_sum(stream ? (cudaStream_t)stream : g_dev.stream, d_points, (int)k, d_out);
+  bops->jacobian_sum(pick_stream(stream), d_points, (int)k, d_out);
   {
     std::lock_guard<std::mutex> lk(g_prof.mu);
     g_prof.launches += 1;
@@ -759,7 +805,7 @@ int b200_ck_setup_synthetic(int curve_id, const void* gen_affine, uint64_t k0, s
   if (curve_id < 0 || curve_id > 3) return fail(B200_E_ARG, "unknown curve id %d", curve_id);
   if (!gen_affine || !handle || n == 0) return fail(B200_E_ARG, "bad argument");
   size_t total = n + (with_h ? 1 : 0);
-  dev_buf bases, gen;
+  dev_buf bases(g_dev.stream), gen(g_dev.stream);
   if ((rc = bases.alloc(total * 64))) return rc;
   if ((rc = gen.alloc(64))) return rc;
   CU(cudaMemcpyAsync(gen.p, gen_affine, 64, cudaMemcpyHostToDevice, g_dev.stream));
@@ -785,7 +831,7 @@ int b200_ck_setup_tau(int curve_id, const void* gen_affine, const void* tau_mont
   if (rc) return rc;
   if (curve_id < 0 || curve_id > 3) return fail(B200_E_ARG, "unknown curve id %d", curve_id);
   if (!gen_affine || !tau_mont || !handle || n == 0) return fail(B200_E_ARG, "bad argument");
-  dev_buf bases, gen, tau, pw;
+  dev_buf bases(g_dev.stream), gen(g_dev.stream), tau(g_dev.stream), pw(g_dev.stream);
   if ((rc = bases.alloc(n * 64)) || (rc = gen.alloc(64)) || (rc = tau.alloc(32)) || (rc = pw.alloc(n * 32))) return rc;
   CU(cudaMemcpyAsync(gen.p, gen_affine, 64, cudaMemcpyHostToDevice, g_dev.stream));
   CU(cudaMemcpyAsync(tau.p, tau_mont, 32, cudaMemcpyHostToDevice, g_dev.stream));
@@ -1032,8 +1078,7 @@ int b200_msm_dev(uint64_t handle, size_t base_offset, const void* d_scalars, siz
   std::lock_guard<std::mutex> lk(t.mu);
   rc = ensure_workspace(t, n ? n : 1, 1);
   if (rc) return rc;
-  return enqueue_msm(t, base_offset, d_scalars, n, d_out,
-                     stream ? (cudaStream_t)stream : g_dev.stream);
+  return enqueue_msm(t, base_offset, d_scalars, n, d_out, pick_stream(stream));
 }
 
 int b200_commit_dev(uint64_t handle, const void* d_scalars, size_t n, const void* d_blind_or_null,
@@ -1050,7 +1095,7 @@ int b200_commit_dev(uint64_t handle, const void* d_scalars, size_t n, const void
   std::lock_guard<std::mutex> lk(t.mu);
   rc = ensure_workspace(t, n + 1, 1);
   if (rc) return rc;
-  cudaStream_t s = stream ? (cudaStream_t)stream : g_dev.stream;
+  cudaStream_t s = pick_stream(stream);
   if (!d_blind_or_null) return enqueue_msm(t, 0, d_scalars, n, d_out, s);
   if ((rc = ws_acquire(t.ws, s))) return rc;
   // the blinding scalar must follow the vector in one buffer: stage both in the workspace
@@ -1147,8 +1192,7 @@ int b200_commit_many_dev(uint64_t handle, const void* const* d_scalars, const si
   if (!d_out) return fail(B200_E_ARG, "null pointer");
   if ((rc = check_many(*ck, d_scalars, lens, k))) return rc;
   std::lock_guard<std::mutex> lk(ck->mu);
-  return enqueue_many(*ck, d_scalars, lens, k, /*from_host=*/false, d_out,
-                      stream ? (cudaStream_t)stream : g_dev.stream);
+  return enqueue_many(*ck, d_scalars, lens, k, /*from_host=*/false, d_out, pick_stream(stream));
 }
 
 int b200_msm_many_dev(uint64_t handle, const size_t* base_offsets, const void* const* d_scalars, const size_t* lens,
@@ -1167,7 +1211,7 @@ int b200_msm_many_dev(uint64_t handle, const size_t* base_offsets, const void* c
   }
   std::lock_guard<std::mutex> lk(ck->mu);
   return enqueue_many(*ck, d_scalars, lens, k, /*from_host=*/false, d_out,
-                      stream ? (cudaStream_t)stream : g_dev.stream, base_offsets);
+                      pick_stream(stream), base_offsets);
 }
 
 int b200_msm_small(uint64_t handle, size_t base_offset, const void* scalars, int elem_bytes, size_t n,
@@ -1388,8 +1432,7 @@ int b200_msm_sharded_dev(uint64_t handle, size_t base_offset, const void* d_scal
   if (rc) return rc;
   msm_peer peer = g->desc;
   peer.epoch = ++g->desc.epoch;
-  return enqueue_msm(t, t.ws, base_offset, d_scalars, n, d_out, stream ? (cudaStream_t)stream : g_dev.stream, 0,
-                     false, false, &peer);
+  return enqueue_msm(t, t.ws, base_offset, d_scalars, n, d_out, pick_stream(stream), 0, false, false, &peer);
 #endif
 }
 
@@ -1465,36 +1508,29 @@ int b200_poseidon_ro_dev(uint64_t handle, const void* d_elems, size_t n, int num
   if (!d_out96 || (n && !d_elems)) return fail(B200_E_ARG, "null pointer");
   if (num_bits < 1 || num_bits > 250) return fail(B200_E_ARG, "num_bits %d outside 1..250", num_bits);
   if (n >= (1u << 31)) return fail(B200_E_ARG, "too many elements");
-  cudaStream_t s = stream ? (cudaStream_t)stream : g_dev.stream;
+  cudaStream_t s = pick_stream(stream);
   unsigned char tag[32];
   poseidon_tag((uint32_t)n, tag);
-  void* d_tag = nullptr;  // stream-ordered scratch for the 32-byte tag
-  CU(cudaMallocAsync(&d_tag, 32, s));
-  CU(cudaMemcpyAsync(d_tag, tag, 32, cudaMemcpyHostToDevice, s));  // (pageable source: staged before the call returns)
-  ops_for_field(c->fid)->poseidon_ro(s, c->t, c->r_f, c->r_p, c->rc, c->mds, d_elems, (uint32_t)n, d_tag, num_bits,
+  dev_buf d_tag(s);
+  if ((rc = d_tag.alloc(32))) return rc;
+  CU(cudaMemcpyAsync(d_tag.p, tag, 32, cudaMemcpyHostToDevice, s));  // (pageable source: staged before the call returns)
+  ops_for_field(c->fid)->poseidon_ro(s, c->t, c->r_f, c->r_p, c->rc, c->mds, d_elems, (uint32_t)n, d_tag.p, num_bits,
                                      start_with_one, d_out96);
   count_launch(1);
   CU(cudaGetLastError());
-  CU(cudaFreeAsync(d_tag, s));
   return B200_OK;
 }
 int b200_poseidon_ro(uint64_t handle, const void* elems_mont, size_t n, int num_bits, int start_with_one, void* out96) {
   int rc = ensure_init();
   if (rc) return rc;
-  if (!out96 || (n && !elems_mont)) return fail(B200_E_ARG, "null pointer");
-  dev_buf in, out;
-  if ((rc = in.alloc(n * 32 + 32)) || (rc = out.alloc(96))) return rc;
-  if (n) CU(cudaMemcpyAsync(in.p, elems_mont, n * 32, cudaMemcpyHostToDevice, g_dev.stream));
-  rc = b200_poseidon_ro_dev(handle, in.p, n, num_bits, start_with_one, out.p, g_dev.stream);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(out96, out.p, 96, cudaMemcpyDeviceToHost, g_dev.stream));
-  CU(cudaStreamSynchronize(g_dev.stream));
-  return B200_OK;
+  return via_device({up(elems_mont, 32 * n), down(out96, 96)}, [&](void* const* d, cudaStream_t s) {
+    return b200_poseidon_ro_dev(handle, d[0], n, num_bits, start_with_one, d[1], s);
+  });
 }
 int b200_to_mont_dev(int fid, const void* d_canonical, size_t n, void* d_out, void* stream) {
   return with_field(fid, [&](const field_ops* ops) {
     if (n && (!d_canonical || !d_out)) return fail(B200_E_ARG, "null pointer");
-    ops->to_mont(stream ? (cudaStream_t)stream : g_dev.stream, d_canonical, n, d_out);
+    ops->to_mont(pick_stream(stream), d_canonical, n, d_out);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1719,7 +1755,7 @@ int b200_cross_term_dev(int fid, const void* az, const void* bz, const void* cz,
   return with_field(fid, [&](const field_ops* ops) {
     if (n == 0) return (int)B200_OK;
     if (!az || !bz || !cz || !e1 || !u || !t) return fail(B200_E_ARG, "null pointer");
-    ops->cross_term(stream ? (cudaStream_t)stream : g_dev.stream, az, bz, cz, e1, e2, u, n, t);
+    ops->cross_term(pick_stream(stream), az, bz, cz, e1, e2, u, n, t);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1730,7 +1766,7 @@ int b200_axpy_dev(int fid, const void* a, const void* b, const void* r, size_t n
   return with_field(fid, [&](const field_ops* ops) {
     if (n == 0) return (int)B200_OK;
     if (!a || !b || !r || !out) return fail(B200_E_ARG, "null pointer");
-    ops->axpy(stream ? (cudaStream_t)stream : g_dev.stream, a, b, r, n, out);
+    ops->axpy(pick_stream(stream), a, b, r, n, out);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1740,7 +1776,7 @@ int b200_vec_mul_dev(int fid, const void* a, const void* b, size_t n, void* out,
   return with_field(fid, [&](const field_ops* ops) {
     if (n == 0) return (int)B200_OK;
     if (!a || !b || !out) return fail(B200_E_ARG, "null pointer");
-    ops->vec_mul(stream ? (cudaStream_t)stream : g_dev.stream, a, b, n, out);
+    ops->vec_mul(pick_stream(stream), a, b, n, out);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1751,7 +1787,7 @@ int b200_logup_hash_dev(int fid, const void* val, const void* addr_or_null, cons
   return with_field(fid, [&](const field_ops* ops) {
     if (n == 0) return (int)B200_OK;
     if (!val || !gamma || !r || !out) return fail(B200_E_ARG, "null pointer");
-    ops->logup_hash(stream ? (cudaStream_t)stream : g_dev.stream, val, addr_or_null, gamma, r, n, out);
+    ops->logup_hash(pick_stream(stream), val, addr_or_null, gamma, r, n, out);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1761,7 +1797,7 @@ int b200_vec_add_dev(int fid, const void* a, const void* b, size_t n, void* out,
   return with_field(fid, [&](const field_ops* ops) {
     if (n == 0) return (int)B200_OK;
     if (!a || !b || !out) return fail(B200_E_ARG, "null pointer");
-    ops->vec_add(stream ? (cudaStream_t)stream : g_dev.stream, a, b, n, out);
+    ops->vec_add(pick_stream(stream), a, b, n, out);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1772,7 +1808,7 @@ int b200_bind_top_dev(int fid, void* z, size_t n, const void* r, void* stream) {
     if (n < 2) return (int)B200_OK;
     if (n & 1) return fail(B200_E_ARG, "bind_top needs an even length, got %zu", n);
     if (!z || !r) return fail(B200_E_ARG, "null pointer");
-    ops->bind_top(stream ? (cudaStream_t)stream : g_dev.stream, z, n, r);
+    ops->bind_top(pick_stream(stream), z, n, r);
     count_launch(1);
     CU(cudaGetLastError());
     return (int)B200_OK;
@@ -1784,7 +1820,7 @@ int b200_bind_top_multi_dev(int fid, void* const* zs, size_t k, size_t n, const 
     if (k == 0 || n < 2) return (int)B200_OK;
     if (n & 1) return fail(B200_E_ARG, "bind_top needs an even length, got %zu", n);
     if (!zs || !r) return fail(B200_E_ARG, "null pointer");
-    cudaStream_t s = stream ? (cudaStream_t)stream : g_dev.stream;
+    cudaStream_t s = pick_stream(stream);
     for (size_t j = 0; j < k; j += BIND_MULTI_MAX) {
       const int cnt = (int)(k - j < (size_t)BIND_MULTI_MAX ? k - j : (size_t)BIND_MULTI_MAX);
       for (int i = 0; i < cnt; i++)
@@ -1797,94 +1833,41 @@ int b200_bind_top_multi_dev(int fid, void* const* zs, size_t k, size_t n, const 
   });
 }
 
-// host-pointer forms: upload, run, download
+// host-pointer forms: the _dev forms above, staged through via_device
 int b200_cross_term(int fid, const void* az, const void* bz, const void* cz, const void* e1,
                     const void* e2, const void* u, size_t n, void* t) {
   int rc = ensure_init();
-  if (rc) return rc;
-  if (n == 0) return B200_OK;
-  if (!az || !bz || !cz || !e1 || !u || !t) return fail(B200_E_ARG, "null pointer");
-  dev_buf buf;
-  size_t vec = n * 32;
-  int nvec = e2 ? 6 : 5;
-  rc = buf.alloc(vec * nvec + 32);
-  if (rc) return rc;
-  char* d = (char*)buf.p;
-  cudaStream_t s = g_dev.stream;
-  const void* src[5] = {az, bz, cz, e1, e2};
-  for (int k = 0; k < (e2 ? 5 : 4); k++)
-    CU(cudaMemcpyAsync(d + vec * k, src[k], vec, cudaMemcpyHostToDevice, s));
-  char* du = d + vec * nvec;
-  CU(cudaMemcpyAsync(du, u, 32, cudaMemcpyHostToDevice, s));
-  char* dt = d + vec * (nvec - 1);
-  rc = b200_cross_term_dev(fid, d, d + vec, d + 2 * vec, d + 3 * vec, e2 ? d + 4 * vec : nullptr, du,
-                           n, dt, s);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(t, dt, vec, cudaMemcpyDeviceToHost, s));
-  CU(cudaStreamSynchronize(s));
-  return B200_OK;
+  if (rc || n == 0) return rc;
+  const size_t vec = 32 * n;
+  return via_device({up(az, vec), up(bz, vec), up(cz, vec), up(e1, vec), up(e2, vec), up(u, 32), down(t, vec)},
+                    [&](void* const* d, cudaStream_t s) {
+                      return b200_cross_term_dev(fid, d[0], d[1], d[2], d[3], d[4], d[5], n, d[6], s);
+                    });
 }
 
 int b200_axpy(int fid, const void* a, const void* b, const void* r, size_t n, void* out) {
   int rc = ensure_init();
-  if (rc) return rc;
-  if (n == 0) return B200_OK;
-  if (!a || !b || !r || !out) return fail(B200_E_ARG, "null pointer");
-  dev_buf buf;
-  size_t vec = n * 32;
-  rc = buf.alloc(vec * 3 + 32);
-  if (rc) return rc;
-  char* d = (char*)buf.p;
-  cudaStream_t s = g_dev.stream;
-  CU(cudaMemcpyAsync(d, a, vec, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(d + vec, b, vec, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(d + 3 * vec, r, 32, cudaMemcpyHostToDevice, s));
-  rc = b200_axpy_dev(fid, d, d + vec, d + 3 * vec, n, d + 2 * vec, s);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(out, d + 2 * vec, vec, cudaMemcpyDeviceToHost, s));
-  CU(cudaStreamSynchronize(s));
-  return B200_OK;
+  if (rc || n == 0) return rc;
+  return via_device({up(a, 32 * n), up(b, 32 * n), up(r, 32), down(out, 32 * n)}, [&](void* const* d, cudaStream_t s) {
+    return b200_axpy_dev(fid, d[0], d[1], d[2], n, d[3], s);
+  });
 }
 
 int b200_vec_add(int fid, const void* a, const void* b, size_t n, void* out) {
   int rc = ensure_init();
-  if (rc) return rc;
-  if (n == 0) return B200_OK;
-  if (!a || !b || !out) return fail(B200_E_ARG, "null pointer");
-  dev_buf buf;
-  size_t vec = n * 32;
-  rc = buf.alloc(vec * 3);
-  if (rc) return rc;
-  char* d = (char*)buf.p;
-  cudaStream_t s = g_dev.stream;
-  CU(cudaMemcpyAsync(d, a, vec, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(d + vec, b, vec, cudaMemcpyHostToDevice, s));
-  rc = b200_vec_add_dev(fid, d, d + vec, n, d + 2 * vec, s);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(out, d + 2 * vec, vec, cudaMemcpyDeviceToHost, s));
-  CU(cudaStreamSynchronize(s));
-  return B200_OK;
+  if (rc || n == 0) return rc;
+  return via_device({up(a, 32 * n), up(b, 32 * n), down(out, 32 * n)}, [&](void* const* d, cudaStream_t s) {
+    return b200_vec_add_dev(fid, d[0], d[1], n, d[2], s);
+  });
 }
 
+// in place: all n elements go up, the bound first half comes back
 int b200_bind_top(int fid, void* z, size_t n, const void* r) {
   int rc = ensure_init();
-  if (rc) return rc;
-  if (n < 2) return B200_OK;
-  if (n & 1) return fail(B200_E_ARG, "bind_top needs an even length, got %zu", n);
-  if (!z || !r) return fail(B200_E_ARG, "null pointer");
-  dev_buf buf;
-  size_t vec = n * 32;
-  rc = buf.alloc(vec + 32);
-  if (rc) return rc;
-  char* d = (char*)buf.p;
-  cudaStream_t s = g_dev.stream;
-  CU(cudaMemcpyAsync(d, z, vec, cudaMemcpyHostToDevice, s));
-  CU(cudaMemcpyAsync(d + vec, r, 32, cudaMemcpyHostToDevice, s));
-  rc = b200_bind_top_dev(fid, d, n, d + vec, s);
-  if (rc) return rc;
-  CU(cudaMemcpyAsync(z, d, vec / 2, cudaMemcpyDeviceToHost, s));
-  CU(cudaStreamSynchronize(s));
-  return B200_OK;
+  if (rc || n < 2) return rc;
+  return via_device({{z, 32 * n, z, 16 * n, 0}, up(r, 32)}, [&](void* const* d, cudaStream_t s) {
+    return b200_bind_top_dev(fid, d[0], n, d[1], s);
+  });
 }
 
 }  // extern "C"
