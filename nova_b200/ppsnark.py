@@ -23,8 +23,8 @@ from .native import check, lib
 from .provider import CommitmentKey, _cbuf, _jac_to_affine
 from .spartan import (SC_CUBIC, SC_EQ_CUBIC2, SC_EQ_CUBIC2_M1, SC_EQ_CUBIC3, SC_EQ_CUBIC3_M1, SC_EQ_QUAD1,
                       SC_EQ_QUAD1_M1, SC_LINEAR, SC_NOUT, SC_QUADRATIC, DeviceVec, EqSumCheckInstance,
-                      SparseMatrix, UniPoly, _challenge_dev, _sc_eval_dev, _small_buf, commit_many_dev,
-                      update_claim)
+                      SparseMatrix, SumcheckProof, UniPoly, _bind_all, _challenge_dev, _sc_eval_dev, _small_buf,
+                      commit_many_dev, update_claim)
 
 
 SCB_RAW3, SCB_LIN2, SCB_EQ_DEG2, SCB_EQ_DEG1 = range(4)  # b200_scb_desc.kind (include/nova_b200.h)
@@ -170,13 +170,6 @@ class RoundSums:
         return res
 
 
-def _bind_all(fid, polys, length, r_dev):
-    """bind_poly_var_top of several tables of one length with the same challenge: ONE launch (b200_bind_top_multi_dev)"""
-    polys = list(polys)
-    ptrs = (ctypes.c_void_p * len(polys))(*[Z.ptr.value for Z in polys])
-    check(lib().b200_bind_top_multi_dev(fid, ptrs, len(polys), length, r_dev.ptr, None))
-
-
 def commit_dev(curve, ck: CommitmentKey, v, n: int):
     """CE::commit(ck, v, r = 0) of a device-resident vector -> affine (x, y) or None."""
     out = DeviceVec(96)
@@ -290,110 +283,6 @@ def memory_compute_oracles(fid, r: int, gamma: int, N: int, mem_row, addr_row, L
 
 
 # ---- the three engines ---------------------------------------------------------------------------
-class MemorySumcheckInstance:
-    shard = None  # a Shard while prove_helper_sharded runs the sharded rounds on this engine
-
-    def __init__(self, fid, N, polys_oracle, polys_aux, rhos, ts_row, ts_col):
-        self.fid, self.p, self.len = fid, fields.MODULUS[fid], N
-        self.t_inv_row, self.w_inv_row, self.t_inv_col, self.w_inv_col = (dev_copy(v, N) for v in polys_oracle)
-        self.t_row, self.w_row, self.t_col, self.w_col = polys_aux  # consumed (moved in the reference)
-        self.ts_row, self.ts_col = dev_copy(ts_row, N), dev_copy(ts_col, N)
-        self.eq = EqSumCheckInstance(fid, rhos)
-        self.running = [0] * 6
-        self.saved = [[0, 0, 0] for _ in range(6)]
-
-    def initial_claims(self):
-        return [0] * 6
-
-    def size(self):
-        return self.len
-
-    def enqueue(self, sums: RoundSums):
-        L, R, sh = self.eq._tables()
-        n = self.len
-        self._slots = [
-            sums.add(SC_LINEAR, self.t_inv_row, self.w_inv_row, None, n),
-            sums.add(SC_LINEAR, self.t_inv_col, self.w_inv_col, None, n),
-            sums.add(SC_EQ_CUBIC3, self.t_inv_row, self.t_row, self.ts_row, n, L, R, sh),
-            sums.add(SC_EQ_CUBIC2, self.w_inv_row, self.w_row, None, n, L, R, sh),
-            sums.add(SC_EQ_CUBIC3, self.t_inv_col, self.t_col, self.ts_col, n, L, R, sh),
-            sums.add(SC_EQ_CUBIC2, self.w_inv_col, self.w_col, None, n, L, R, sh),
-        ]
-
-    def _derived(self, j, t0, tinf):
-        d = self.eq._derive(t0, tinf, self.running[j], True)
-        if d is not None:
-            return list(d)
-        # tau = 0: third sum (sumcheck.rs:1082-1178)
-        L, R, sh = self.eq._tables()
-        A, B, C, form = {2: (self.t_inv_row, self.t_row, self.ts_row, SC_EQ_CUBIC3_M1),
-                         3: (self.w_inv_row, self.w_row, None, SC_EQ_CUBIC2_M1),
-                         4: (self.t_inv_col, self.t_col, self.ts_col, SC_EQ_CUBIC3_M1),
-                         5: (self.w_inv_col, self.w_col, None, SC_EQ_CUBIC2_M1)}[j]
-        (tm1,) = _sc_eval_one(self.shard, self.fid, form, A, B, C, self.len, L, R, sh)
-        e0, slope, em1 = self.eq.eq_tau_0_a_inf[self.eq.round - 1]
-        q, p = self.eq.eval_eq_left, self.p
-        return [e0 * q * t0 % p, slope * q * tinf % p, em1 * q * tm1 % p]
-
-    def evaluation_points(self, res):
-        s = self._slots
-        self.saved = [[res[s[0]][0], 0, res[s[0]][1]], [res[s[1]][0], 0, res[s[1]][1]]]
-        for j in range(2, 6):
-            self.saved.append(self._derived(j, res[s[j]][0], res[s[j]][1]))
-        return [list(e) for e in self.saved]
-
-    def bound(self, r, r_dev):
-        self.running = [update_claim(self.p, self.running[j], self.saved[j], r) for j in range(6)]
-        _bind_all(self.fid, [self.t_row, self.t_inv_row, self.w_row, self.w_inv_row, self.ts_row, self.t_col,
-                             self.t_inv_col, self.w_col, self.w_inv_col, self.ts_col], self.len, r_dev)
-        self.len //= 2
-        self.eq.bound(r)
-
-    TABLES = ("t_row", "t_inv_row", "w_row", "w_inv_row", "ts_row", "t_col", "t_inv_col", "w_col", "w_inv_col", "ts_col")
-
-    # -- device-transcript loop (prove_helper_device): claim kinds, third sums for tau = 0, binds only --
-    KINDS = (SCB_LIN2, SCB_LIN2, SCB_EQ_DEG2, SCB_EQ_DEG2, SCB_EQ_DEG2, SCB_EQ_DEG2)
-    # per claim: (sum form, third-sum form, tables A / B / C) -- what enqueue / enqueue_m1 launch, as data
-    PROGRAM = ((SC_LINEAR, -1, ("t_inv_row", "w_inv_row", None)),
-               (SC_LINEAR, -1, ("t_inv_col", "w_inv_col", None)),
-               (SC_EQ_CUBIC3, SC_EQ_CUBIC3_M1, ("t_inv_row", "t_row", "ts_row")),
-               (SC_EQ_CUBIC2, SC_EQ_CUBIC2_M1, ("w_inv_row", "w_row", None)),
-               (SC_EQ_CUBIC3, SC_EQ_CUBIC3_M1, ("t_inv_col", "t_col", "ts_col")),
-               (SC_EQ_CUBIC2, SC_EQ_CUBIC2_M1, ("w_inv_col", "w_col", None)))
-
-    def eq_instances(self):
-        return [self.eq]
-
-    def claim_eq(self):
-        return [None, None, 0, 0, 0, 0]
-
-    def running_claims(self):
-        return list(self.running)
-
-    def enqueue_m1(self, sums: RoundSums):
-        """t(-1) of the four eq-weighted claims (sumcheck.rs:1082-1178), for a round whose tau is 0."""
-        L, R, sh = self.eq._tables()
-        n = self.len
-        return [None, None,
-                sums.add(SC_EQ_CUBIC3_M1, self.t_inv_row, self.t_row, self.ts_row, n, L, R, sh),
-                sums.add(SC_EQ_CUBIC2_M1, self.w_inv_row, self.w_row, None, n, L, R, sh),
-                sums.add(SC_EQ_CUBIC3_M1, self.t_inv_col, self.t_col, self.ts_col, n, L, R, sh),
-                sums.add(SC_EQ_CUBIC2_M1, self.w_inv_col, self.w_col, None, n, L, R, sh)]
-
-    def slots(self):
-        return list(self._slots)
-
-    def bound_device(self, r_dev):
-        _bind_all(self.fid, [self.t_row, self.t_inv_row, self.w_row, self.w_inv_row, self.ts_row, self.t_col,
-                             self.t_inv_col, self.w_col, self.w_inv_col, self.ts_col], self.len, r_dev)
-        self.len //= 2
-        self.eq.round += 1
-
-    def final_claims(self):
-        g = lambda name: _final(self, name)
-        return [[g("t_inv_row"), g("w_inv_row"), g("ts_row")], [g("t_inv_col"), g("w_inv_col"), g("ts_col")]]
-
-
 def _read1(view) -> bytes:
     out = ctypes.create_string_buffer(32)
     check(lib().b200_memcpy_d2h(out, view.ptr, 32))
@@ -404,186 +293,157 @@ def _first(fid, v) -> int:
     return fields.unpack(fid, _read1(v))[0]
 
 
-def _final(eng, name: str) -> int:
-    """element 0 of a fully bound table: from the values b200_sumcheck_batched returned, else read from the device"""
-    got = getattr(eng, "_finals", None)
-    return got[name] if got is not None and name in got else _first(eng.fid, getattr(eng, name))
+class _Engine:
+    """One engine of the batched sum-check (ppsnark.rs:886-983), stated once as data by its subclass:
 
+      CLAIMS  one row per claim: (b200_scb_desc kind SCB_*, sum form, third-sum form for a round whose tau is 0 or -1,
+              the names of the three tables it reads (None for an unused one), the index of its eq instance in
+              `eqs` or None)
+      TABLES  every table, in bind order
+      FINALS  the final claims, as groups of table names
 
-class InnerBatchedSumcheckInstance:
-    shard = None
+    The constructor calls `_setup`.  The round's launches, the evaluation points, the binds and the final claims of the
+    host loop, and the claims as data for the device loops, all follow from these three."""
+    shard = None  # a Shard while prove_helper runs the rounds on this rank's shards of the tables
 
-    def __init__(self, fid, N, claim, L_row, L_col, val, claim_E, r_outer, E):
-        p = fields.MODULUS[fid]
-        self.fid, self.p, self.len = fid, p, N
-        self.claim, self.claim_E = claim % p, claim_E % p
-        self.L_row, self.L_col, self.val, self.E = dev_copy(L_row, N), dev_copy(L_col, N), val, dev_copy(E, N)
-        self.eq = EqSumCheckInstance(fid, r_outer)
-        self.running_E, self.saved_E = claim_E % p, [0, 0, 0]
+    def _setup(self, fid, n, claims, eqs=()):
+        self.fid, self.p, self.len = fid, fields.MODULUS[fid], n
+        self.claims = [c % self.p for c in claims]
+        self.eqs = list(eqs)
+        # running claims are needed by the eq claims only (their evaluation points); 0 for the others
+        self.running = [c if row[4] is not None else 0 for c, row in zip(self.claims, self.CLAIMS)]
+        self._finals = {}  # table name -> final value, when b200_sumcheck_batched returned them
 
-    def initial_claims(self):
-        return [self.claim, self.claim_E]
-
-    def size(self):
-        return self.len
+    def _add(self, sums, form, names, g, tabs):
+        A, B, C = (None if t is None else getattr(self, t) for t in names)
+        return sums.add(form, A, B, C, self.len, *(() if g is None else tabs[g]))
 
     def enqueue(self, sums: RoundSums):
-        L, R, sh = self.eq._tables()
-        self._slots = [sums.add(SC_CUBIC, self.L_row, self.L_col, self.val, self.len),
-                       sums.add(SC_EQ_QUAD1, self.E, None, None, self.len, L, R, sh)]
+        tabs = [q._tables() for q in self.eqs]
+        self.slots = [self._add(sums, form, names, g, tabs) for _, form, _, names, g in self.CLAIMS]
+
+    def enqueue_m1(self, sums: RoundSums) -> list:
+        """the third sums t(-1) of the eq claims whose tau is 0 in this round (sumcheck.rs:1082-1213): a slot or None
+        per claim"""
+        tabs = [q._tables() for q in self.eqs]
+        zero = [q.taus[q.round - 1] % self.p == 0 for q in self.eqs]
+        return [self._add(sums, form_m1, names, g, tabs) if g is not None and zero[g] else None
+                for _, _, form_m1, names, g in self.CLAIMS]
+
+    def _third_sum(self, form, names, g) -> int:
+        A, B, C = (None if t is None else getattr(self, t) for t in names)
+        return _sc_eval_one(self.shard, self.fid, form, A, B, C, self.len, *self.eqs[g]._tables())[0]
 
     def evaluation_points(self, res):
-        e0, bc, einf = res[self._slots[0]]
-        (t0,) = res[self._slots[1]]
-        d = self.eq._derive(t0, 0, self.running_E, False)
-        if d is None:  # tau = 0 (sumcheck.rs:1180-1213)
-            L, R, sh = self.eq._tables()
-            (tm1,) = _sc_eval_one(self.shard, self.fid, SC_EQ_QUAD1_M1, self.E, None, None, self.len, L, R, sh)
-            q0, _, qm1 = self.eq.eq_tau_0_a_inf[self.eq.round - 1]
-            q = self.eq.eval_eq_left
-            d = (q0 * q * t0 % self.p, 0, qm1 * q * tm1 % self.p)
-        self.saved_E = list(d)
-        return [[e0, bc, einf], [d[0], 0, d[2]]]
+        """[e(0), lead, e(-1)] per claim from the round's sums `res` (indexed by the slots `enqueue` took)"""
+        self.saved = []
+        for (kind, _, form_m1, names, g), k, claim in zip(self.CLAIMS, self.slots, self.running):
+            r = res[k]
+            if kind == SCB_LIN2:
+                ev = (r[0], 0, r[1])
+            elif kind == SCB_RAW3:
+                ev = tuple(r)
+            else:  # SCB_EQ_DEG2: r = (t0, tinf); SCB_EQ_DEG1: r = (t0,)
+                ev = self.eqs[g].evaluation_points(r[0], r[1] if kind == SCB_EQ_DEG2 else 0, claim,
+                                                   lambda: self._third_sum(form_m1, names, g))
+            self.saved.append(ev)
+        return [list(ev) for ev in self.saved]
+
+    def _bind(self, r_dev):
+        _bind_all(self.fid, [getattr(self, t) for t in self.TABLES], self.len, r_dev)
+        self.len //= 2
 
     def bound(self, r, r_dev):
-        self.running_E = update_claim(self.p, self.running_E, self.saved_E, r)
-        _bind_all(self.fid, [self.L_row, self.L_col, self.val, self.E], self.len, r_dev)
-        self.len //= 2
-        self.eq.bound(r)
-
-    TABLES = ("L_row", "L_col", "val", "E")
-    KINDS = (SCB_RAW3, SCB_EQ_DEG1)
-    PROGRAM = ((SC_CUBIC, -1, ("L_row", "L_col", "val")), (SC_EQ_QUAD1, SC_EQ_QUAD1_M1, ("E", None, None)))
-
-    def eq_instances(self):
-        return [self.eq]
-
-    def claim_eq(self):
-        return [None, 0]
-
-    def running_claims(self):
-        return [0, self.running_E]
-
-    def enqueue_m1(self, sums: RoundSums):
-        L, R, sh = self.eq._tables()
-        return [None, sums.add(SC_EQ_QUAD1_M1, self.E, None, None, self.len, L, R, sh)]
-
-    def slots(self):
-        return list(self._slots)
+        self.running = [0 if row[4] is None else update_claim(self.p, c, ev, r)
+                        for c, ev, row in zip(self.running, self.saved, self.CLAIMS)]
+        self._bind(r_dev)
+        for q in self.eqs:
+            q.bound(r)
 
     def bound_device(self, r_dev):
-        _bind_all(self.fid, [self.L_row, self.L_col, self.val, self.E], self.len, r_dev)
-        self.len //= 2
-        self.eq.round += 1
+        """the binds of a round whose algebra ran on the device"""
+        self._bind(r_dev)
+        for q in self.eqs:
+            q.round += 1
 
     def final_claims(self):
-        return [[_final(self, "L_row"), _final(self, "L_col")], [_final(self, "E")]]
+        """element 0 of the fully bound tables: from the values b200_sumcheck_batched returned, else read from the device"""
+        got = self._finals
+        return [[got[t] if t in got else _first(self.fid, getattr(self, t)) for t in group] for group in self.FINALS]
 
 
-class WitnessBoundSumcheck:
-    shard = None
+class MemorySumcheckInstance(_Engine):
+    CLAIMS = ((SCB_LIN2, SC_LINEAR, -1, ("t_inv_row", "w_inv_row", None), None),
+              (SCB_LIN2, SC_LINEAR, -1, ("t_inv_col", "w_inv_col", None), None),
+              (SCB_EQ_DEG2, SC_EQ_CUBIC3, SC_EQ_CUBIC3_M1, ("t_inv_row", "t_row", "ts_row"), 0),
+              (SCB_EQ_DEG2, SC_EQ_CUBIC2, SC_EQ_CUBIC2_M1, ("w_inv_row", "w_row", None), 0),
+              (SCB_EQ_DEG2, SC_EQ_CUBIC3, SC_EQ_CUBIC3_M1, ("t_inv_col", "t_col", "ts_col"), 0),
+              (SCB_EQ_DEG2, SC_EQ_CUBIC2, SC_EQ_CUBIC2_M1, ("w_inv_col", "w_col", None), 0))
+    TABLES = ("t_row", "t_inv_row", "w_row", "w_inv_row", "ts_row", "t_col", "t_inv_col", "w_col", "w_inv_col", "ts_col")
+    FINALS = (("t_inv_row", "w_inv_row", "ts_row"), ("t_inv_col", "w_inv_col", "ts_col"))
+
+    def __init__(self, fid, N, polys_oracle, polys_aux, rhos, ts_row, ts_col):
+        self.t_inv_row, self.w_inv_row, self.t_inv_col, self.w_inv_col = (dev_copy(v, N) for v in polys_oracle)
+        self.t_row, self.w_row, self.t_col, self.w_col = polys_aux  # consumed (moved in the reference)
+        self.ts_row, self.ts_col = dev_copy(ts_row, N), dev_copy(ts_col, N)
+        self._setup(fid, N, [0] * 6, [EqSumCheckInstance(fid, rhos)])
+
+
+class InnerBatchedSumcheckInstance(_Engine):
+    CLAIMS = ((SCB_RAW3, SC_CUBIC, -1, ("L_row", "L_col", "val"), None),
+              (SCB_EQ_DEG1, SC_EQ_QUAD1, SC_EQ_QUAD1_M1, ("E", None, None), 0))
+    TABLES = ("L_row", "L_col", "val", "E")
+    FINALS = (("L_row", "L_col"), ("E",))
+
+    def __init__(self, fid, N, claim, L_row, L_col, val, claim_E, r_outer, E):
+        self.L_row, self.L_col, self.val, self.E = dev_copy(L_row, N), dev_copy(L_col, N), val, dev_copy(E, N)
+        self._setup(fid, N, [claim, claim_E], [EqSumCheckInstance(fid, r_outer)])
+
+
+class WitnessBoundSumcheck(_Engine):
+    CLAIMS = ((SCB_LIN2, SC_QUADRATIC, -1, ("masked_eq", "W", None), None),)
+    TABLES = ("W", "masked_eq")
+    FINALS = (("W", "masked_eq"),)
 
     def __init__(self, fid, N, tau: list, W_padded, num_vars: int):
         m = num_vars.bit_length() - 1
         assert m < N.bit_length() - 1  # ppsnark.rs:288
-        self.fid, self.len = fid, N
         self.W = dev_copy(W_padded, N)
         self.masked_eq = DeviceVec(32 * N)
         self._tau_dev = DeviceVec.from_bytes(fields.pack(fid, tau))  # kept: the eq kernels read it asynchronously
         check(lib().b200_eq_table_dev(fid, self._tau_dev.ptr, len(tau), self.masked_eq.ptr, None))
         check(lib().b200_memset_dev(self.masked_eq.ptr, 0, 32 << m, None))  # first 2^m entries -> 0
-
-    def initial_claims(self):
-        return [0]
-
-    def size(self):
-        return self.len
-
-    def enqueue(self, sums: RoundSums):
-        self._slot = sums.add(SC_QUADRATIC, self.masked_eq, self.W, None, self.len)
-
-    def evaluation_points(self, res):
-        e0, einf = res[self._slot]
-        return [[e0, 0, einf]]
-
-    def bound(self, r, r_dev):
-        _bind_all(self.fid, [self.W, self.masked_eq], self.len, r_dev)
-        self.len //= 2
-
-    TABLES = ("W", "masked_eq")
-    KINDS = (SCB_LIN2,)
-    PROGRAM = ((SC_QUADRATIC, -1, ("masked_eq", "W", None)),)
+        self._setup(fid, N, [0])
 
     @classmethod
     def from_shards(cls, fid, n_local: int, W_local, masked_eq_local):
         """this rank's cyclic shard of W (padded) and of the masked eq table (ppsnark.rs:270-300)"""
         self = cls.__new__(cls)
-        self.fid, self.len = fid, n_local
         self.W, self.masked_eq = dev_copy(W_local, n_local), dev_copy(masked_eq_local, n_local)
+        self._setup(fid, n_local, [0])
         return self
 
-    def eq_instances(self):
-        return []
 
-    def claim_eq(self):
-        return [None]
-
-    def running_claims(self):
-        return [0]
-
-    def enqueue_m1(self, sums: RoundSums):
-        return [None]
-
-    def slots(self):
-        return [self._slot]
-
-    def bound_device(self, r_dev):
-        _bind_all(self.fid, [self.W, self.masked_eq], self.len, r_dev)
-        self.len //= 2
-
-    def final_claims(self):
-        return [[_final(self, "W"), _final(self, "masked_eq")]]
-
-
-def prove_helper(fid, mem, inner, witness, transcript):
-    """RelaxedR1CSSNARK::prove_helper (ppsnark.rs:886-983)."""
+def _batching(fid, engines, transcript):
+    """ppsnark.rs:909-921: the engines' initial claims combined with the powers of s -> (coefficients, combined claim)"""
     p = fields.MODULUS[fid]
-    assert mem.size() == inner.size() == witness.size()
-    claims = mem.initial_claims() + inner.initial_claims() + witness.initial_claims()
+    assert len({eng.len for eng in engines}) == 1
+    claims = [c for eng in engines for c in eng.claims]
     s = transcript.squeeze(b"r")
     coeffs = [pow(s, i, p) for i in range(len(claims))]
-    e = sum(c * k for c, k in zip(claims, coeffs)) % p
-    rs, polys = [], []
-    sums = RoundSums(fid)
-    for _ in range(mem.size().bit_length() - 1):
-        for eng in (mem, inner, witness):
-            eng.enqueue(sums)
-        res = sums.fetch()
-        evals = mem.evaluation_points(res) + inner.evaluation_points(res) + witness.evaluation_points(res)
-        assert len(evals) == len(claims)
-        c0 = sum(evals[i][0] * coeffs[i] for i in range(len(evals))) % p
-        cb = sum(evals[i][1] * coeffs[i] for i in range(len(evals))) % p
-        ci = sum(evals[i][2] * coeffs[i] for i in range(len(evals))) % p
-        poly = UniPoly.from_evals_deg3(p, [c0, (e - c0) % p, cb, ci])
-        transcript.absorb_bytes(b"p", poly.to_transcript_bytes())
-        r = transcript.squeeze(b"c")
-        rs.append(r)
-        r_dev = _challenge_dev(fid, r)
-        for eng in (mem, inner, witness):
-            eng.bound(r, r_dev)
-        e = poly.evaluate(r)
-        polys.append(poly.compress())
-    return polys, rs, mem.final_claims(), inner.final_claims(), witness.final_claims()
+    return coeffs, sum(c * k for c, k in zip(claims, coeffs)) % p
 
 
-def prove_helper_sharded(fid, mem, inner, witness, transcript, rank: int, world: int, gather):
-    """`prove_helper` (ppsnark.rs:886-983) with the sixteen tables sharded CYCLICALLY over `world` ranks (a power
-    of two): the engines are built from this rank's shards (local length N / world; the eq instances from the
-    full point).  Per round every rank reduces its shard (nine sums; the eq weight uses the global index), the
-    partial sums are exchanged with ONE all-gather (`gather(bytes) -> list of every rank's bytes`), the O(1)
-    algebra and the transcript run replicated, and the binds need no exchange (i and i + len/2 are co-resident
-    under the cyclic layout).  When one element per rank is left the tables are all-gathered (16 x world
-    elements) and the last log2(world) rounds run replicated.  Every rank returns what `prove_helper` returns."""
+def prove_helper(fid, mem, inner, witness, transcript, rank: int = 0, world: int = 1, gather=None):
+    """RelaxedR1CSSNARK::prove_helper (ppsnark.rs:886-983).
+
+    With `world` > 1 (a power of two) the sixteen tables are sharded CYCLICALLY over `world` ranks: the engines are
+    built from this rank's shards (local length N / world; the eq instances from the full point).  Per round every rank
+    reduces its shard (nine sums; the eq weight uses the global index), the partial sums are exchanged with ONE
+    all-gather (`gather(bytes) -> list of every rank's bytes`), the O(1) algebra and the transcript run replicated, and
+    the binds need no exchange (i and i + len/2 are co-resident under the cyclic layout).  When one element per rank is
+    left the tables are all-gathered (16 x world elements) and the last log2(world) rounds run replicated.  Every rank
+    returns what the unsharded loop returns."""
     p = fields.MODULUS[fid]
     assert world & (world - 1) == 0
     engines = (mem, inner, witness)
@@ -600,12 +460,8 @@ def prove_helper_sharded(fid, mem, inner, witness, transcript, rank: int, world:
                 setattr(eng, name, DeviceVec.from_bytes(b"".join(gather(_read1(old)))))
             eng.len = world
 
-    assert mem.size() == inner.size() == witness.size()
-    n_rounds = (mem.size() * world).bit_length() - 1
-    claims = mem.initial_claims() + inner.initial_claims() + witness.initial_claims()
-    s = transcript.squeeze(b"r")
-    coeffs = [pow(s, i, p) for i in range(len(claims))]
-    e = sum(c * k for c, k in zip(claims, coeffs)) % p
+    n_rounds = (mem.len * world).bit_length() - 1
+    coeffs, e = _batching(fid, engines, transcript)
     rs, polys = [], []
     shard = Shard(rank, world, reduce) if world > 1 else None
     sums = RoundSums(fid, shard=shard)
@@ -613,7 +469,7 @@ def prove_helper_sharded(fid, mem, inner, witness, transcript, rank: int, world:
         eng.shard = shard
     try:
         for _ in range(n_rounds):
-            if shard is not None and mem.size() == 1:
+            if shard is not None and mem.len == 1:
                 replicate_tail()
                 shard = sums.shard = None
                 for eng in engines:
@@ -621,7 +477,7 @@ def prove_helper_sharded(fid, mem, inner, witness, transcript, rank: int, world:
             for eng in engines:
                 eng.enqueue(sums)
             res = sums.fetch()
-            evals = mem.evaluation_points(res) + inner.evaluation_points(res) + witness.evaluation_points(res)
+            evals = [ev for eng in engines for ev in eng.evaluation_points(res)]
             c0 = sum(evals[i][0] * coeffs[i] for i in range(len(evals))) % p
             cb = sum(evals[i][1] * coeffs[i] for i in range(len(evals))) % p
             ci = sum(evals[i][2] * coeffs[i] for i in range(len(evals))) % p
@@ -640,74 +496,64 @@ def prove_helper_sharded(fid, mem, inner, witness, transcript, rank: int, world:
     return polys, rs, mem.final_claims(), inner.final_claims(), witness.final_claims()
 
 
+# the name the sharded callers know: prove_helper_sharded(fid, mem, inner, witness, transcript, rank, world, gather)
+prove_helper_sharded = prove_helper
+
+
+def _device_claims(fid, engines, transcript):
+    """What both device loops start from: the number of rounds, the coefficients and the combined claim
+    (`_batching`), every claim as (engine, CLAIMS row, its eq instance numbered across the engines or None), the eq
+    instances in that numbering, and the running claims."""
+    coeffs, e = _batching(fid, engines, transcript)
+    claims, eqs = [], []
+    for eng in engines:
+        claims += [(eng, row, None if row[4] is None else len(eqs) + row[4]) for row in eng.CLAIMS]
+        eqs += eng.eqs
+    assert len(claims) <= SCB_MAX_CLAIMS and len(eqs) <= SCB_MAX_EQ
+    running = [c for eng in engines for c in eng.running]
+    return engines[0].len.bit_length() - 1, coeffs, e, claims, eqs, running
+
+
 def prove_helper_device(fid, mem, inner, witness, transcript):
-    """prove_helper (ppsnark.rs:886-983) as ONE library call (b200_sumcheck_batched): the engines describe their
-    claims as data (PROGRAM / KINDS / claim_eq), the library runs every round -- all sums in two launches, the round
-    kernel, one bind launch, the short rounds inside one kernel -- and the proof is read back once.
+    """prove_helper (ppsnark.rs:886-983) as ONE library call (b200_sumcheck_batched): the engines' claims as data
+    (b200_scp_program), the library runs every round -- all sums in two launches, the round kernel, one bind launch,
+    the short rounds inside one kernel -- and the proof is read back once.
     `transcript` needs the serialisable fields `round`, `state`, `buf` (see spartan._device_loop)."""
-    p = fields.MODULUS[fid]
     engines = (mem, inner, witness)
-    assert mem.size() == inner.size() == witness.size()
-    nr = mem.size().bit_length() - 1
-    claims = mem.initial_claims() + inner.initial_claims() + witness.initial_claims()
-    k = len(claims)
-    assert k <= SCB_MAX_CLAIMS
-    s = transcript.squeeze(b"r")
-    coeffs = [pow(s, i, p) for i in range(k)]
-    e = sum(c * cl for c, cl in zip(claims, coeffs)) % p
+    nr, coeffs, e, claims, eqs, running = _device_claims(fid, engines, transcript)
     prog = ScpProgram()
     tables, index = [], {}
-    eqs = []
-    i = 0
-    for eng in engines:
-        base = len(eqs)
-        eqs += eng.eq_instances()
-        for (form, form_m1, names), kind, g in zip(eng.PROGRAM, eng.KINDS, eng.claim_eq()):
-            prog.kind[i], prog.form[i], prog.form_m1[i] = kind, form, form_m1
-            prog.eq_of[i] = -1 if g is None else base + g
-            for c, name in enumerate(names):
-                if name is None:
-                    prog.tab[i][c] = -1
-                    continue
-                key = (id(eng), name)
-                if key not in index:
-                    index[key] = len(tables)
-                    tables.append(getattr(eng, name))
-                prog.tab[i][c] = index[key]
-            i += 1
-        for name in eng.TABLES:  # tables no claim reads are still bound every round (none today)
-            if (id(eng), name) not in index:
-                index[(id(eng), name)] = len(tables)
-                tables.append(getattr(eng, name))
-    assert i == k and len(tables) <= SCP_MAX_TABLES and len(eqs) <= SCB_MAX_EQ
-    prog.nclaims, prog.neq, prog.ntables, prog.num_rounds = k, len(eqs), len(tables), nr
+
+    def table(eng, name):
+        if (eng, name) not in index:
+            index[(eng, name)] = len(tables)
+            tables.append(getattr(eng, name))
+        return index[(eng, name)]
+    for i, (eng, (kind, form, form_m1, names, _), g) in enumerate(claims):
+        prog.kind[i], prog.form[i], prog.form_m1[i] = kind, form, form_m1
+        prog.eq_of[i] = -1 if g is None else g
+        for c, name in enumerate(names):
+            prog.tab[i][c] = -1 if name is None else table(eng, name)
+    for eng in engines:  # tables no claim reads are still bound every round (none today)
+        for name in eng.TABLES:
+            table(eng, name)
+    assert len(tables) <= SCP_MAX_TABLES
+    prog.nclaims, prog.neq, prog.ntables, prog.num_rounds = len(claims), len(eqs), len(tables), nr
     for t, Z in enumerate(tables):
         prog.tables[t] = Z.ptr.value
     tau_bufs = [_cbuf(fields.pack(fid, q.taus)) for q in eqs]
     for g, buf in enumerate(tau_bufs):
         prog.taus[g] = ctypes.addressof(buf)
-    running = [x for eng in engines for x in eng.running_claims()]
-    tr = (ctypes.c_ubyte * 72)()
-    ctypes.memmove(tr, int(transcript.round).to_bytes(8, "little") + bytes(transcript.state), 72)
-    pending = bytes(transcript.buf)
-    polys_raw, rs_raw = ctypes.create_string_buffer(96 * nr), ctypes.create_string_buffer(32 * nr)
-    finals = ctypes.create_string_buffer(32 * len(tables))
-    check(lib().b200_sumcheck_batched(fid, ctypes.byref(prog), _cbuf(fields.pack(fid, coeffs)),
-                                      _cbuf(fields.to_mont_bytes(fid, e)), _cbuf(fields.pack(fid, running)), tr,
-                                      _cbuf(pending) if pending else None, len(pending), polys_raw, rs_raw, finals))
-    raw = bytes(tr)
-    transcript.round = int.from_bytes(raw[:8], "little")
-    transcript.state = raw[8:72]
-    transcript.buf = b""
-    vals = fields.unpack(fid, finals.raw)
+    inputs = (_cbuf(fields.pack(fid, coeffs)), _cbuf(fields.to_mont_bytes(fid, e)), _cbuf(fields.pack(fid, running)))
+    polys, rs, vals = SumcheckProof._device_loop(
+        fid, transcript, lambda *io: lib().b200_sumcheck_batched(fid, ctypes.byref(prog), *inputs, *io), nr, 3,
+        len(tables))
     for eng in engines:
         eng.len = 1
-        eng._finals = {name: vals[t] for (owner, name), t in index.items() if owner == id(eng)}  # read by final_claims
-        for q in eng.eq_instances():
+        eng._finals = {name: vals[t] for (owner, name), t in index.items() if owner is eng}
+        for q in eng.eqs:
             q.round += nr
-    coeffs_out = [int.from_bytes(polys_raw.raw[32 * i:32 * i + 32], "little") for i in range(3 * nr)]
-    polys = [coeffs_out[3 * j:3 * j + 3] for j in range(nr)]
-    return polys, fields.unpack(fid, rs_raw.raw), mem.final_claims(), inner.final_claims(), witness.final_claims()
+    return polys, rs, mem.final_claims(), inner.final_claims(), witness.final_claims()
 
 
 def prove_helper_device_rounds(fid, mem, inner, witness, transcript):
@@ -718,22 +564,7 @@ def prove_helper_device_rounds(fid, mem, inner, witness, transcript):
     `transcript` needs the serialisable fields `round`, `state`, `buf` (see spartan._device_loop)."""
     p = fields.MODULUS[fid]
     engines = (mem, inner, witness)
-    assert mem.size() == inner.size() == witness.size()
-    nr = mem.size().bit_length() - 1
-    claims = mem.initial_claims() + inner.initial_claims() + witness.initial_claims()
-    k = len(claims)
-    assert k <= SCB_MAX_CLAIMS
-    s = transcript.squeeze(b"r")
-    coeffs = [pow(s, i, p) for i in range(k)]
-    e = sum(c * cl for c, cl in zip(claims, coeffs)) % p
-    kinds = [kd for eng in engines for kd in eng.KINDS]
-    eqs, eq_of = [], []
-    for eng in engines:  # global numbering of the eq instances
-        base = len(eqs)
-        eqs += eng.eq_instances()
-        eq_of += [None if g is None else base + g for g in eng.claim_eq()]
-    assert len(eqs) <= SCB_MAX_EQ
-    running = [x for eng in engines for x in eng.running_claims()]
+    nr, coeffs, e, claims, eqs, running = _device_claims(fid, engines, transcript)
     pad = lambda xs, n: list(xs) + [0] * (n - len(xs))
     head = (fields.to_mont_bytes(fid, e) + bytes(32) + int(transcript.round).to_bytes(8, "little")
             + bytes(transcript.state) + bytes(8))
@@ -750,23 +581,14 @@ def prove_helper_device_rounds(fid, mem, inner, witness, transcript):
     for j in range(nr):
         for eng in engines:
             eng.enqueue(sums)
-        slots = [sl for eng in engines for sl in eng.slots()]
-        m1 = [None] * k
-        off = 0
-        for eng in engines:  # third sums for the eq instances whose tau is 0 in this round
-            qs = eng.eq_instances()
-            if any(q.taus[q.round - 1] % p == 0 for q in qs):
-                got = eng.enqueue_m1(sums)
-                for i, g in enumerate(eng.claim_eq()):
-                    if g is not None and qs[g].taus[qs[g].round - 1] % p == 0:
-                        m1[off + i] = got[i]
-            off += len(eng.KINDS)
+        slots = [sl for eng in engines for sl in eng.slots]
+        m1 = [sl for eng in engines for sl in eng.enqueue_m1(sums)]  # third sums for the eq instances whose tau is 0
         d = ScbDesc()
-        d.nclaims, d.neq = k, len(eqs)
-        for i in range(k):
-            d.kind[i], d.slot[i] = kinds[i], 3 * slots[i]
+        d.nclaims, d.neq = len(claims), len(eqs)
+        for i, (_, row, g) in enumerate(claims):
+            d.kind[i], d.slot[i] = row[0], 3 * slots[i]
             d.slot_m1[i] = -1 if m1[i] is None else 3 * m1[i]
-            d.eq_of[i] = -1 if eq_of[i] is None else eq_of[i]
+            d.eq_of[i] = -1 if g is None else g
         for g, q in enumerate(eqs):
             d.tau[g] = tau_dev[g].ptr.value + 32 * (q.round - 1)
             d.tau_inv[g] = tinv_dev[g].ptr.value + 32 * (q.round - 1)
@@ -784,25 +606,6 @@ def prove_helper_device_rounds(fid, mem, inner, witness, transcript):
     coeffs_out = [int.from_bytes(raw_polys[32 * i:32 * i + 32], "little") for i in range(3 * nr)]
     polys = [coeffs_out[3 * j:3 * j + 3] for j in range(nr)]
     return polys, fields.unpack(fid, raw_rs), mem.final_claims(), inner.final_claims(), witness.final_claims()
-
-
-def _prove_cubic3_resident(fid, claim, taus, A, B, C, length, transcript):
-    """SumcheckProof::prove_cubic_with_three_inputs (sumcheck.rs:446-507) on resident vectors."""
-    p = fields.MODULUS[fid]
-    eq = EqSumCheckInstance(fid, taus)
-    rs, polys = [], []
-    for _ in range(len(taus)):
-        e0, lead, em1 = eq.evaluation_points_cubic_with_three_inputs(A, B, C, length, claim)
-        poly = UniPoly.from_evals_deg3(p, [e0, (claim - e0) % p, lead, em1])
-        transcript.absorb_bytes(b"p", poly.to_transcript_bytes())
-        r = transcript.squeeze(b"c")
-        rs.append(r)
-        polys.append(poly.compress())
-        claim = poly.evaluate(r)
-        _bind_all(fid, (A, B, C), length, _challenge_dev(fid, r))
-        eq.bound(r)
-        length //= 2
-    return polys, rs, [_first(fid, Z) for Z in (A, B, C)]
 
 
 def _mle_eval(fid, Z, ell, r_dev) -> int:
@@ -852,11 +655,9 @@ def prove_core(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: 
     uCz_E = DeviceVec(32 * num_cons)
     check(lib().b200_axpy_dev(fid, Ed.ptr, Cz.ptr, u_dev.ptr, num_cons, uCz_E.ptr, None))  # E + u*Cz
     mark("spmv")
-    if device_transcript:  # one call, transcript on the device (b200_sumcheck_cubic3)
-        from .spartan import SumcheckProof
-        sc_outer, r_outer, claims_outer = SumcheckProof.prove_cubic_with_three_inputs_device(fid, 0, tau, Az, Bz, uCz_E, tr)
-    else:
-        sc_outer, r_outer, claims_outer = _prove_cubic3_resident(fid, 0, tau, Az, Bz, uCz_E, num_cons, tr)
+    outer = (SumcheckProof.prove_cubic_with_three_inputs_device if device_transcript  # one call (b200_sumcheck_cubic3)
+             else SumcheckProof.prove_cubic_with_three_inputs)
+    sc_outer, r_outer, claims_outer = outer(fid, 0, tau, Az, Bz, uCz_E, tr)
     eAz, eBz = claims_outer[0], claims_outer[1]
     eCz = _mle_eval(fid, Cz, nro, DeviceVec.from_bytes(fields.pack(fid, r_outer)))
     eE_outer = (claims_outer[2] - U["u"] * eCz) % p
@@ -960,10 +761,12 @@ def prove(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: dict,
     return out
 
 
-def _rlc_dev(fid, polys, coeffs, n, out):
+def _rlc_dev(fid, polys, coeffs, n, out, lens=None):
+    """out[0..n) = sum_i coeffs[i] polys[i], polynomial i read over its first lens[i] entries (default n) and
+    zero-extended"""
     k = len(polys)
     ptrs = (ctypes.c_void_p * k)(*[v.ptr.value for v in polys])
-    lens = (ctypes.c_size_t * k)(*([n] * k))
+    lens = (ctypes.c_size_t * k)(*([n] * k if lens is None else lens))
     cd = DeviceVec.from_bytes(fields.pack(fid, coeffs))
     check(lib().b200_rlc_dev(fid, ptrs, lens, k, cd.ptr, n, out.ptr, None))
     check(lib().b200_sync())  # `cd` and the pointer table must outlive the launch

@@ -22,12 +22,9 @@ as E::TE is in the reference (needs `absorb_bytes`, `squeeze` and the serialisab
 """
 from __future__ import annotations
 
-import ctypes
-
 from . import fields
 from .native import check, lib
-from .ppsnark import (View, _as_dev, _mle_eval, _prove_cubic3_resident, _rlc_dev, commitment_transcript_bytes,
-                      dev_scalar, dev_zeros, to_repr)
+from .ppsnark import View, _as_dev, _mle_eval, _rlc_dev, commitment_transcript_bytes, dev_scalar, dev_zeros, to_repr
 from .provider import CommitmentKey, Curve, DlogGroup, _cbuf
 from .spartan import DeviceVec, SumcheckProof
 
@@ -78,10 +75,9 @@ def prove_core(curve, ck: CommitmentKey | None, S: dict, U: dict, W: dict, vk_di
     uCz_E = DeviceVec(32 * num_cons)
     check(lib().b200_axpy_dev(fid, Ed.ptr, Cz.ptr, u_dev.ptr, num_cons, uCz_E.ptr, None))  # E + u*Cz
     mark("spmv")
-    if device_transcript:
-        sc_outer, r_x, claims_outer = SumcheckProof.prove_cubic_with_three_inputs_device(fid, 0, tau, Az, Bz, uCz_E, tr)
-    else:
-        sc_outer, r_x, claims_outer = _prove_cubic3_resident(fid, 0, tau, Az, Bz, uCz_E, num_cons, tr)
+    outer = (SumcheckProof.prove_cubic_with_three_inputs_device if device_transcript
+             else SumcheckProof.prove_cubic_with_three_inputs)
+    sc_outer, r_x, claims_outer = outer(fid, 0, tau, Az, Bz, uCz_E, tr)
     claim_Az, claim_Bz = claims_outer[0], claims_outer[1]
     rx_dev = DeviceVec.from_bytes(fields.pack(fid, r_x))
     claim_Cz = _mle_eval(fid, Cz, nrx, rx_dev)
@@ -98,10 +94,8 @@ def prove_core(curve, ck: CommitmentKey | None, S: dict, U: dict, W: dict, vk_di
     poly_ABC = DeviceVec(32 * 2 * num_vars)
     _rlc_dev(fid, tabs, [1, r, r * r % p], 2 * num_vars, poly_ABC)
     mark("eval_tables")
-    if device_transcript:
-        sc_inner, r_y, _ = SumcheckProof.prove_quad_prod_device(fid, claim_inner_joint, nry, poly_ABC, z, tr)
-    else:
-        sc_inner, r_y, _ = _prove_quad_prod_resident(fid, claim_inner_joint, nry, poly_ABC, z, tr)
+    inner = SumcheckProof.prove_quad_prod_device if device_transcript else SumcheckProof.prove_quad_prod
+    sc_inner, r_y, _ = inner(fid, claim_inner_joint, nry, poly_ABC, z, tr)
     eval_W = _mle_eval(fid, Wd, nry - 1, DeviceVec.from_bytes(fields.pack(fid, r_y[1:])))
     tr.absorb_bytes(b"w", to_repr(eval_W))
     mark("inner_sumcheck")
@@ -128,40 +122,11 @@ def prove_core(curve, ck: CommitmentKey | None, S: dict, U: dict, W: dict, vk_di
         fields.pack(fid, coeffs), b"".join(_affine_bytes(curve, cm) for (cm, _, _) in u_vec))
     size_max = max(num_vars, num_cons)
     batched_poly = DeviceVec(32 * size_max)  # PolyEvalWitness::batch_diff_size, mod.rs:165-222
-    _rlc_diff(fid, [Wd, Ed], [num_vars, num_cons], coeffs, size_max, batched_poly)
+    _rlc_dev(fid, [Wd, Ed], coeffs, size_max, batched_poly, lens=[num_vars, num_cons])
     mark("batch_eval_reduce")
     return dict(sc_proof_outer=sc_outer, claims_outer=(claim_Az, claim_Bz, claim_Cz), eval_E=eval_E,
                 sc_proof_inner=sc_inner, eval_W=eval_W, sc_proof_batch=sc_batch, evals_batch=evals_batch,
                 r_x=r_x, r_y=r_y, batched_c=batched_c, batched_x=r_b, batched_e=batched_e, batched_poly=batched_poly)
-
-
-def _rlc_diff(fid, polys, lens, coeffs, n, out):
-    k = len(polys)
-    ptrs = (ctypes.c_void_p * k)(*[v.ptr.value for v in polys])
-    ls = (ctypes.c_size_t * k)(*lens)
-    cd = DeviceVec.from_bytes(fields.pack(fid, coeffs))
-    check(lib().b200_rlc_dev(fid, ptrs, ls, k, cd.ptr, n, out.ptr, None))
-    check(lib().b200_sync())  # `cd` and the pointer table must outlive the launch
-
-
-def _prove_quad_prod_resident(fid, claim, num_rounds, A: DeviceVec, B: DeviceVec, transcript):
-    """SumcheckProof::prove_quad_prod (sumcheck.rs:199-242) on resident vectors, host transcript."""
-    from .spartan import SC_QUAD_PROD, UniPoly, _bind_dev, _sc_eval_dev
-    p = fields.MODULUS[fid]
-    length = 1 << num_rounds
-    rs, polys = [], []
-    for _ in range(num_rounds):
-        e0, bc = _sc_eval_dev(fid, SC_QUAD_PROD, A, B, None, length, None, None, 0)
-        poly = UniPoly.from_evals_deg2(p, [e0, (claim - e0) % p, bc])
-        transcript.absorb_bytes(b"p", poly.to_transcript_bytes())
-        r = transcript.squeeze(b"c")
-        rs.append(r)
-        polys.append(poly.compress())
-        claim = poly.evaluate(r)
-        _bind_dev(fid, A, length, r)
-        _bind_dev(fid, B, length, r)
-        length //= 2
-    return polys, rs, fields.unpack(fid, A.to_bytes(32)) + fields.unpack(fid, B.to_bytes(32))
 
 
 def prove(curve, ck: CommitmentKey, S: dict, U: dict, W: dict, vk_digest: int, transcript, device_transcript: bool = True,

@@ -311,6 +311,18 @@ def _bind_dev(fid, Z: DeviceVec, length: int, r_int: int):
     check(lib().b200_bind_top_dev(fid, Z.ptr, length, _challenge_dev(fid, r_int).ptr, None))
 
 
+def _bind_all(fid, polys, length, r_dev):
+    """bind_poly_var_top of several tables of one length with the same challenge: ONE launch (b200_bind_top_multi_dev)"""
+    polys = list(polys)
+    ptrs = (ctypes.c_void_p * len(polys))(*[Z.ptr.value for Z in polys])
+    check(lib().b200_bind_top_multi_dev(fid, ptrs, len(polys), length, r_dev.ptr, None))
+
+
+def _resident(x) -> DeviceVec:
+    """a DeviceVec as it is (the caller's table is bound in place), bytes uploaded into a new one"""
+    return x if isinstance(x, DeviceVec) else DeviceVec.from_bytes(x)
+
+
 class EqSumCheckInstance:
     """sumcheck.rs:593-1251.  The sqrt-sized eq tables are built on the host exactly as in `new`
     (:606-664) and uploaded once; per-round sums run on the device."""
@@ -349,40 +361,35 @@ class EqSumCheckInstance:
             return self._left[self.first_half - self.round], self._right[self.second_half], self.second_half
         return None, self._right[self.init_num_vars - self.round], 0  # :1248-1251
 
-    def _derive(self, t0, tinf, claim, deg2: bool):
+    def evaluation_points(self, t0, tinf, claim, t_m1):
+        """(s(0), lead, s(-1)) of the eq-weighted claim `claim` from the sums t(0), t(inf) of its inner polynomial
+        (tinf = 0 when that polynomial is linear).  s(-1) comes from t(1), which the claim determines unless this
+        round's tau is 0 (sumcheck.rs:696-698); then `t_m1()` is called for the third sum t(-1)
+        (sumcheck.rs:1082-1213)."""
         p, q = self.p, self.eval_eq_left
         e0, slope, em1 = self.eq_tau_0_a_inf[self.round - 1]
+        s0 = e0 * q * t0 % p
         l1p = (e0 + slope) * q % p
         if l1p == 0:
-            return None  # tau = 0: caller computes the third sum (sumcheck.rs:696-698)
-        s0 = e0 * q * t0 % p
-        t1 = (claim - s0) * pow(l1p, -1, p) % p
-        if deg2:
-            return s0, slope * q * tinf % p, em1 * q * ((2 * tinf + 2 * t0 - t1) % p) % p
-        return s0, 0, em1 * q * ((2 * t0 - t1) % p) % p
+            tm1 = t_m1()
+        else:
+            t1 = (claim - s0) * pow(l1p, -1, p) % p
+            tm1 = 2 * tinf + 2 * t0 - t1
+        return s0, slope * q * tinf % p, em1 * q * (tm1 % p) % p
 
     def evaluation_points_cubic_with_three_inputs(self, A, B, C, length, claim):
+        """sumcheck.rs:900-966 (+ fall-back :1082-1178)."""
         L, R, sh = self._tables()
         t0, tinf = _sc_eval_dev(self.fid, SC_EQ_CUBIC3, A, B, C, length, L, R, sh)
-        d = self._derive(t0, tinf, claim, True)
-        if d is not None:
-            return d
-        (tm1,) = _sc_eval_dev(self.fid, SC_EQ_CUBIC3_M1, A, B, C, length, L, R, sh)
-        e0, slope, em1 = self.eq_tau_0_a_inf[self.round - 1]
-        q, p = self.eval_eq_left, self.p
-        return e0 * q * t0 % p, slope * q * tinf % p, em1 * q * tm1 % p
+        return self.evaluation_points(t0, tinf, claim,
+                                      lambda: _sc_eval_dev(self.fid, SC_EQ_CUBIC3_M1, A, B, C, length, L, R, sh)[0])
 
     def evaluation_points_quadratic_with_one_input(self, A, length, claim):
         """sumcheck.rs:1039-1080 (+ fall-back :1180-1213)."""
         L, R, sh = self._tables()
         (t0,) = _sc_eval_dev(self.fid, SC_EQ_QUAD1, A, None, None, length, L, R, sh)
-        d = self._derive(t0, 0, claim, False)
-        if d is not None:
-            return d
-        (tm1,) = _sc_eval_dev(self.fid, SC_EQ_QUAD1_M1, A, None, None, length, L, R, sh)
-        e0, _, em1 = self.eq_tau_0_a_inf[self.round - 1]
-        q, p = self.eval_eq_left, self.p
-        return e0 * q * t0 % p, 0, em1 * q * tm1 % p
+        return self.evaluation_points(t0, 0, claim,
+                                      lambda: _sc_eval_dev(self.fid, SC_EQ_QUAD1_M1, A, None, None, length, L, R, sh)[0])
 
     def bound(self, r):
         tau = self.taus[self.round - 1]
@@ -456,11 +463,12 @@ class SumcheckProof:
         return out, rs, finals
 
     @staticmethod
-    def prove_quad_prod(fid, claim, num_rounds, poly_A: bytes, poly_B: bytes, transcript):
-        """sumcheck.rs:199-242 -> (compressed polys, challenges r, [A(r), B(r)])."""
+    def prove_quad_prod(fid, claim, num_rounds, poly_A, poly_B, transcript):
+        """sumcheck.rs:199-242 -> (compressed polys, challenges r, [A(r), B(r)]).  poly_A / poly_B: bytes (uploaded)
+        or DeviceVec of 2^num_rounds entries (bound in place)."""
         p = fields.MODULUS[fid]
-        A, B = DeviceVec.from_bytes(poly_A), DeviceVec.from_bytes(poly_B)
-        length = len(poly_A) // 32
+        length = 1 << num_rounds if isinstance(poly_A, DeviceVec) else len(poly_A) // 32
+        A, B = _resident(poly_A), _resident(poly_B)
         rs, polys = [], []
         for _ in range(num_rounds):
             e0, bc = _sc_eval_dev(fid, SC_QUAD_PROD, A, B, None, length, None, None, 0)
@@ -476,12 +484,12 @@ class SumcheckProof:
         return polys, rs, fields.unpack(fid, A.to_bytes(32)) + fields.unpack(fid, B.to_bytes(32))
 
     @staticmethod
-    def prove_cubic_with_three_inputs(fid, claim, taus, poly_A: bytes, poly_B: bytes, poly_C: bytes,
-                                      transcript):
-        """sumcheck.rs:446-507."""
+    def prove_cubic_with_three_inputs(fid, claim, taus, poly_A, poly_B, poly_C, transcript):
+        """sumcheck.rs:446-507.  poly_A / poly_B / poly_C: bytes (uploaded) or DeviceVec of 2^len(taus) entries
+        (bound in place)."""
         p = fields.MODULUS[fid]
-        A, B, C = (DeviceVec.from_bytes(x) for x in (poly_A, poly_B, poly_C))
-        length = len(poly_A) // 32
+        length = 1 << len(taus) if isinstance(poly_A, DeviceVec) else len(poly_A) // 32
+        A, B, C = (_resident(x) for x in (poly_A, poly_B, poly_C))
         eq = EqSumCheckInstance(fid, taus)
         rs, polys = [], []
         for _ in range(len(taus)):
@@ -492,8 +500,7 @@ class SumcheckProof:
             rs.append(r)
             polys.append(poly.compress())
             claim = poly.evaluate(r)
-            for Z in (A, B, C):
-                _bind_dev(fid, Z, length, r)
+            _bind_all(fid, (A, B, C), length, _challenge_dev(fid, r))
             eq.bound(r)
             length //= 2
         finals = [fields.unpack(fid, Z.to_bytes(32))[0] for Z in (A, B, C)]
@@ -528,13 +535,7 @@ class SumcheckProof:
             return [sum(a * v[c] for a, v in zip(alphas, per)) % p for c in range(nout)]
         for _ in range(len(taus)):
             t0, tinf = sums(SC_EQ_CUBIC3, 2)
-            d = eq._derive(t0, tinf, claim, True)
-            if d is None:  # tau = 0 (sumcheck.rs:838-890)
-                (tm1,) = sums(SC_EQ_CUBIC3_M1, 1)
-                e0c, slope, em1c = eq.eq_tau_0_a_inf[eq.round - 1]
-                q = eq.eval_eq_left
-                d = (e0c * q * t0 % p, slope * q * tinf % p, em1c * q * tm1 % p)
-            e0, lead, em1 = d
+            e0, lead, em1 = eq.evaluation_points(t0, tinf, claim, lambda: sums(SC_EQ_CUBIC3_M1, 1)[0])  # tau = 0: :838-890
             poly = UniPoly.from_evals_deg3(p, [e0, (claim - e0) % p, lead, em1])
             transcript.absorb_bytes(b"p", poly.to_transcript_bytes())
             r = transcript.squeeze(b"c")
@@ -576,8 +577,7 @@ class SumcheckProof:
     def prove_quad_prod_device(fid, claim, num_rounds, poly_A, poly_B, transcript):
         """sumcheck.rs:199-242 through b200_sumcheck_quad_prod.  poly_A / poly_B: bytes (uploaded) or
         DeviceVec (bound in place)."""
-        A = poly_A if isinstance(poly_A, DeviceVec) else DeviceVec.from_bytes(poly_A)
-        B = poly_B if isinstance(poly_B, DeviceVec) else DeviceVec.from_bytes(poly_B)
+        A, B = _resident(poly_A), _resident(poly_B)
         cl = _cbuf(fields.to_mont_bytes(fid, claim))
         return SumcheckProof._device_loop(
             fid, transcript,
@@ -589,7 +589,7 @@ class SumcheckProof:
     def prove_cubic_with_three_inputs_device(fid, claim, taus, poly_A, poly_B, poly_C, transcript):
         """sumcheck.rs:446-507 through b200_sumcheck_cubic3 (eq tables, 1/tau and the tau = 0
         fall-back are handled inside the library)."""
-        A, B, C = (x if isinstance(x, DeviceVec) else DeviceVec.from_bytes(x) for x in (poly_A, poly_B, poly_C))
+        A, B, C = (_resident(x) for x in (poly_A, poly_B, poly_C))
         cl = _cbuf(fields.to_mont_bytes(fid, claim))
         tb = _cbuf(fields.pack(fid, taus))
         return SumcheckProof._device_loop(

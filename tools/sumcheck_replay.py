@@ -85,22 +85,8 @@ def main():
     timed("quad_prod_device_transcript",
           lambda dA, dB, dC: spartan.SumcheckProof.prove_quad_prod_device(fid, 5, l, dA, dB, Transcript(p)))
 
-    def host_cubic(dA, dB, dC):
-        # the existing host loop takes bytes and uploads; time only the loop by handing it resident vectors
-        eq = spartan.EqSumCheckInstance(fid, taus)
-        tr, claim, length = Transcript(p), 5, n
-        for _ in range(l):
-            e0, lead, em1 = eq.evaluation_points_cubic_with_three_inputs(dA, dB, dC, length, claim)
-            poly = spartan.UniPoly.from_evals_deg3(p, [e0, (claim - e0) % p, lead, em1])
-            tr.absorb_bytes(b"p", poly.to_transcript_bytes())
-            r = tr.squeeze(b"c")
-            claim = poly.evaluate(r)
-            for Z in (dA, dB, dC):
-                spartan._bind_dev(fid, Z, length, r)
-            eq.bound(r)
-            length //= 2
-
-    timed("cubic3_host_transcript_python", host_cubic)
+    timed("cubic3_host_transcript_python",
+          lambda dA, dB, dC: spartan.SumcheckProof.prove_cubic_with_three_inputs(fid, 5, taus, dA, dB, dC, Transcript(p)))
 
     # streamed witness commit vs one-shot commit (chunks of 2^16 scalars)
     ck = nb.CommitmentKey.setup_synthetic(nb.Curve(0), n)
