@@ -524,6 +524,15 @@ int b200_spmv_t_dev(uint64_t m_handle, const void* d_rx, size_t out_len, void* d
 /* out[i] = table[idx[i]]: the L_row / L_col oracles of ppsnark (spartan/ppsnark.rs:236-250) */
 int b200_gather(const void* table, size_t table_len, const uint64_t* idx, size_t n, void* out);
 int b200_gather_dev(const void* d_table, const uint32_t* d_idx, size_t n, void* d_out, void* stream);
+/* R1CSShapeSparkRepr::new (spartan/ppsnark.rs:117-190) from the matrices behind three spmv handles (same field,
+ * rows, cols).  N: the caller's next_pow2(max(nnz_A + nnz_B + nnz_C, 2 num_vars, num_cons)); checked to be a
+ * power of two >= total nnz, >= rows, >= cols and < 2^32.  Writes N entries each: d_vecs[0..7) = row, col, val_A,
+ * val_B, val_C, ts_row, ts_col as Montgomery field elements; d_row_idx / d_col_idx = row / col as u32 (the gather
+ * indices).  Padding slots have row 0 and col N - 1.  d_vecs is a host array of device pointers.
+ * Unknown handle: B200_E_HANDLE; mismatched matrices or N not a power of two below 2^32: B200_E_ARG; N too
+ * small: B200_E_RANGE.  Nothing is written on an error. */
+int b200_spark_repr_dev(uint64_t hA, uint64_t hB, uint64_t hC, size_t N, void* const* d_vecs, uint32_t* d_row_idx,
+                        uint32_t* d_col_idx, void* stream);
 /* R1CSShape::multiply_vec / multiply_vec_pair (r1cs/mod.rs:407-471): k matrices, one or two z */
 int b200_spmv_multi(const uint64_t* m_handles, size_t k, const void* z1, const void* z2_or_null,
                     size_t z_len, void* const* out1, void* const* out2_or_null);

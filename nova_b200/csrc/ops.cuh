@@ -15,6 +15,7 @@ struct msm_plan;
 struct multi_args;     // poly_kernels.cuh
 struct poly_multi_args;
 struct scb_tail_args;  // sumcheck_tail.cuh
+struct spark_mats;     // poly_kernels.cuh
 
 struct field_ops {
   int field_id;
@@ -125,6 +126,9 @@ struct field_ops {
                         void* scratch, void* out);
   void (*pow_split_evals)(cudaStream_t, const void* tau, size_t left, size_t right, void* out);
   void (*lerp)(cudaStream_t, const void* a, const void* b, const void* r, size_t n, void* out);
+  // R1CSShapeSparkRepr::new (k_spark_repr): row, col, ts_row, ts_col (Montgomery) and the u32 row / col indices
+  void (*spark_repr)(cudaStream_t, const spark_mats&, size_t N, void* row, void* col, void* ts_row, void* ts_col,
+                     uint32_t* row_idx, uint32_t* col_idx);
 };
 // SM count of the H100 SXM (sm_90a): grids below are sized in whole waves of it
 constexpr int NUM_SMS = 132;

@@ -393,6 +393,10 @@ struct ops_impl {
   static void lerp(cudaStream_t s, const void* a, const void* b, const void* r, size_t n, void* out) {
     k_lerp<F><<<stream_grid(n, 256), 256, 0, s>>>(a, b, r, n, out);
   }
+  static void spark_repr(cudaStream_t s, const spark_mats& m, size_t N, void* row, void* col, void* ts_row,
+                         void* ts_col, uint32_t* row_idx, uint32_t* col_idx) {
+    k_spark_repr<F><<<stream_grid(N, 256), 256, 0, s>>>(m, N, row, col, ts_row, ts_col, row_idx, col_idx);
+  }
   static void spmv_classify(cudaStream_t s, const void* vals, size_t nnz, int8_t* codes) {
     k_spmv_classify<F><<<(unsigned)((nnz + 255) / 256), 256, 0, s>>>(vals, nnz, codes);
   }
@@ -495,7 +499,7 @@ struct ops_impl {
                      powers_canonical, scalar_bases, poseidon_ro, to_mont, exchange_identity,
                      sc_round_batched_fused, sc_reduce_multi_partials, gather_heads, poly_eval_small_multi,
                      eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly,
-                     neutron_evals, pow_split_evals, lerp};
+                     neutron_evals, pow_split_evals, lerp, spark_repr};
   }
 };
 

@@ -861,6 +861,68 @@ static __global__ void __launch_bounds__(256) k_gather32(const void* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------
+// R1CSShapeSparkRepr::new (ppsnark.rs:117-190) from three registered matrices of one shape.
+// Slot i < nnz_A + nnz_B + nnz_C is entry e of matrix k in CSR order; its row is found by binary
+// search in that matrix' indptr.  Padding slots get row 0 and column N - 1 (ppsnark.rs:123).
+// The timestamps need no scatter: ts_row[r] = sum_k (indptr_k[r+1] - indptr_k[r]) and ts_col[c]
+// the same over the CSC pointers tptr_k, plus the N - total padding slots at ts_row[0] and
+// ts_col[N-1].  One thread per slot writes row, col, ts_row and ts_col in Montgomery form and
+// the u32 row / col gather indices.
+// ------------------------------------------------------------------------------------------
+struct spark_mats {
+  const uint32_t* indptr[3];
+  const uint32_t* colidx[3];
+  const uint32_t* tptr[3];
+  size_t nnz[3];
+  size_t rows, cols;
+};
+
+template <class F>
+NOVA_D fe_t fe_from_small(uint64_t x) {
+  fe_t r = fe_zero<F>();
+  r.l[0] = (uint32_t)x;
+  r.l[1] = (uint32_t)(x >> 32);
+  return fe_to_mont<F>(r);
+}
+
+template <class F>
+__global__ void __launch_bounds__(256) k_spark_repr(const spark_mats m, size_t N, void* __restrict__ row,
+                                                    void* __restrict__ col, void* __restrict__ ts_row,
+                                                    void* __restrict__ ts_col, uint32_t* __restrict__ row_idx,
+                                                    uint32_t* __restrict__ col_idx) {
+  const size_t o1 = m.nnz[0], o2 = o1 + m.nnz[1], total = o2 + m.nnz[2], pad = N - total;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < N; i += (size_t)gridDim.x * blockDim.x) {
+    uint32_t r = 0, c = (uint32_t)(N - 1);
+    if (i < total) {
+      const int k = i < o1 ? 0 : (i < o2 ? 1 : 2);
+      const size_t e = i - (k == 0 ? 0 : (k == 1 ? o1 : o2));
+      const uint32_t* ip = k == 0 ? m.indptr[0] : (k == 1 ? m.indptr[1] : m.indptr[2]);
+      const uint32_t* ci = k == 0 ? m.colidx[0] : (k == 1 ? m.colidx[1] : m.colidx[2]);
+      size_t lo = 0, hi = m.rows;  // ip[lo] <= e < ip[hi]
+      while (hi - lo > 1) {
+        const size_t mid = (lo + hi) / 2;
+        if (ip[mid] <= e) lo = mid;
+        else hi = mid;
+      }
+      r = (uint32_t)lo;
+      c = ci[e];
+    }
+    uint64_t tr = i == 0 ? pad : 0, tc = i == N - 1 ? pad : 0;
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+      if (i < m.rows) tr += m.indptr[k][i + 1] - m.indptr[k][i];
+      if (i < m.cols) tc += m.tptr[k][i + 1] - m.tptr[k][i];
+    }
+    row_idx[i] = r;
+    col_idx[i] = c;
+    fe_store(row, i, fe_from_small<F>(r));
+    fe_store(col, i, fe_from_small<F>(c));
+    fe_store(ts_row, i, fe_from_small<F>(tr));
+    fe_store(ts_col, i, fe_from_small<F>(tc));
+  }
+}
+
+// ------------------------------------------------------------------------------------------
 // NeutronNova folding prover pieces (neutron/nifs.rs, spartan/polys/power.rs)
 // ------------------------------------------------------------------------------------------
 // prove_helper (nifs.rs:29-186) before the rho factors.  Row k = i*left + j; with V_t = V1 + t (V2 - V1)

@@ -11,6 +11,7 @@ reference's.  The host keeps the transcript and the O(1) algebra.
 from __future__ import annotations
 
 import ctypes
+import time
 
 from . import fields
 from .native import check, lib
@@ -27,9 +28,13 @@ def commitment_transcript_bytes(P) -> bytes:
 
 class InnerProductArgument:
     @staticmethod
-    def prove(curve, ck: CommitmentKey, comm_a, b_vec: bytes, c_claim: int, a_vec: bytes, transcript):
+    def prove(curve, ck: CommitmentKey, comm_a, b_vec: bytes, c_claim: int, a_vec: bytes, transcript,
+              timings: dict | None = None):
         """`ck` must be registered over the n bases with `h = ck_c` (the single generator the reference
-        keeps in `ck_c`).  b_vec / a_vec are Montgomery field-element vectors of n = 2^l entries."""
+        keeps in `ck_c`).  b_vec / a_vec are Montgomery field-element vectors of n = 2^l entries.
+        `timings`, if given, receives wall-clock seconds summed over the rounds for "ipa_inner_products",
+        "ipa_commit" (the scalar vectors and the two n-point commitments) and "ipa_fold"."""
+        mark = _marker(timings)
         curve = Curve(curve)
         fid = curve.scalar_field
         q = fields.MODULUS[fid]
@@ -63,12 +68,14 @@ class InnerProductArgument:
             check(L.b200_sc_eval_dev(fid, 11, a.ptr, off(b, h), None, h, None, None, 0, ip.ptr, None))
             check(L.b200_sc_eval_dev(fid, 11, off(a, h), b.ptr, None, h, None, None, 0, off(ip, 1), None))
             c_L, c_R = fields.unpack(fid, ip.to_bytes(64))
+            mark("ipa_inner_products")
             check(L.b200_ipa_scalars_dev(fid, a.ptr, w.ptr, n, nk, sL.ptr, sR.ptr, None))
             blind = DeviceVec.from_bytes(fields.pack(fid, [c_L * r0 % q, c_R * r0 % q]))
             check(L.b200_commit_dev(ck.handle, sL.ptr, n, blind.ptr, out.ptr, None))
             check(L.b200_commit_dev(ck.handle, sR.ptr, n, off(blind, 1), ctypes.c_void_p(out.ptr.value + 96), None))
             raw = out.to_bytes(192)
             Lk, Rk = _jac_to_affine(curve, raw[:96]), _jac_to_affine(curve, raw[96:])
+            mark("ipa_commit")
             transcript.absorb_bytes(b"L", commitment_transcript_bytes(Lk))
             transcript.absorb_bytes(b"R", commitment_transcript_bytes(Rk))
             r = transcript.squeeze(b"r")
@@ -83,5 +90,34 @@ class InnerProductArgument:
             L_vec.append(Lk)
             R_vec.append(Rk)
             nk = h
+            mark("ipa_fold")
         a_hat = fields.unpack(fid, a.to_bytes(32))[0]
         return L_vec, R_vec, a_hat
+
+
+def prove_at_point(curve, ck: CommitmentKey, comm, point: list, eval_: int, poly, transcript,
+                   timings: dict | None = None):
+    """EvaluationEngine::prove (ipa_pc.rs:64-77): the inner-product argument between `poly` (2^len(point)
+    Montgomery elements, bytes or DeviceVec) and b_vec = EqPolynomial::new(point).evals(), built on the device.
+    `timings`: "ipa_b_vec" and the phases of InnerProductArgument.prove."""
+    mark = _marker(timings)
+    fid = Curve(curve).scalar_field
+    b_vec = DeviceVec(32 << len(point))
+    x_dev = DeviceVec.from_bytes(fields.pack(fid, point))
+    check(lib().b200_eq_table_dev(fid, x_dev.ptr, len(point), b_vec.ptr, None))
+    mark("ipa_b_vec")
+    return InnerProductArgument.prove(curve, ck, comm, b_vec, eval_, poly, transcript, timings)
+
+
+def _marker(timings: dict | None):
+    """mark(name) adds the seconds since the previous mark to timings[name], the device synchronised first;
+    a no-op without `timings`"""
+    last = [time.perf_counter()]
+
+    def mark(name):
+        if timings is not None:
+            check(lib().b200_sync())
+            now = time.perf_counter()
+            timings[name] = timings.get(name, 0.0) + now - last[0]
+            last[0] = now
+    return mark

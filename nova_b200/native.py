@@ -140,6 +140,7 @@ SIGNATURES = {
     "b200_spmv_t_dev": [c_u64, _P, c_size_t, _P, _P],
     "b200_gather": [_P, c_size_t, ctypes.POINTER(c_u64), c_size_t, _P],
     "b200_gather_dev": [_P, _P, c_size_t, _P, _P],
+    "b200_spark_repr_dev": [c_u64, c_u64, c_u64, c_size_t, ctypes.POINTER(_P), _P, _P, _P],
     "b200_spmv_multi": [ctypes.POINTER(c_u64), c_size_t, _P, _P, c_size_t, ctypes.POINTER(_P),
                         ctypes.POINTER(_P)],
 }

@@ -245,6 +245,27 @@ class SparkRepr:
         self.row_idx, self.col_idx = dev_u32(row), dev_u32(col)
         return self
 
+    @classmethod
+    def from_shape(cls, fid: int, S: dict):
+        """The same representation built on the device from the three registered matrices of `S` (the dict
+        `prove` takes: A/B/C `spartan.SparseMatrix`, num_cons, num_vars) by b200_spark_repr_dev: nothing is
+        read back or uploaded but the pointers."""
+        A, B, C = S["A"], S["B"], S["C"]
+        if any(M.fid != fid for M in (A, B, C)):
+            raise ValueError(f"the matrices are not over field {fid}")
+        self = cls.__new__(cls)
+        N = 1
+        while N < max(A.nnz + B.nnz + C.nnz, 2 * S["num_vars"], S["num_cons"]):
+            N *= 2
+        self.fid, self.N = fid, N
+        vecs = [DeviceVec(32 * N) for _ in range(7)]
+        self.row, self.col, self.val_A, self.val_B, self.val_C, self.ts_row, self.ts_col = vecs
+        self.row_idx, self.col_idx = DeviceVec(4 * N), DeviceVec(4 * N)
+        ptrs = (ctypes.c_void_p * 7)(*[v.ptr.value for v in vecs])
+        check(lib().b200_spark_repr_dev(A.handle, B.handle, C.handle, N, ptrs, self.row_idx.ptr, self.col_idx.ptr,
+                                        None))
+        return self
+
     def evaluation_oracles(self, r_outer_full: list, z, z_len: int):
         """ppsnark.rs:220-253 -> (mem_row, mem_col, L_row, L_col), all of length N on the device."""
         fid, N = self.fid, self.N
@@ -724,6 +745,36 @@ def prove_core(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: 
     return out
 
 
+SHAPE_COMMITMENTS = ("val_A", "val_B", "val_C", "row", "col", "ts_row", "ts_col")  # R1CSShapeSparkCommitment
+
+
+def setup(curve, ck: CommitmentKey, S: dict):
+    """The shape half of ppsnark's setup: R1CSShapeSparkRepr::new + ::commit (ppsnark.rs:117-217), both on the
+    device -> (spark, S_comm).  `S` is the dict `prove` takes, already regular (padding stays the caller's);
+    S_comm maps SHAPE_COMMITMENTS to the commitments (r = 0) of the seven N-element vectors, so `ck` needs N bases."""
+    from .provider import Curve
+    curve = Curve(curve)
+    spark = SparkRepr.from_shape(curve.scalar_field, S)
+    comms = commit_many_dev(curve, ck, [getattr(spark, k) for k in SHAPE_COMMITMENTS], [spark.N] * 7)
+    return spark, dict(zip(SHAPE_COMMITMENTS, comms))
+
+
+def _batched_commitment(curve, U: dict, S_comm: dict, out: dict):
+    """PolyEvalInstance::batch, the commitment part (spartan/mod.rs:346-368): sum_i c^i C_i over the 15 commitments
+    in ppsnark.rs's comm_vec order, c = the batch challenge."""
+    from .provider import DlogGroup
+    from .snark import _affine_bytes
+    fid = curve.scalar_field
+    p = fields.MODULUS[fid]
+    cm = out["comm_mem"]
+    comm_vec = [U["comm_W"], U["comm_E"], out["comm_L_row"], out["comm_L_col"], S_comm["val_A"], S_comm["val_B"],
+                S_comm["val_C"], cm[0], S_comm["row"], cm[1], S_comm["ts_row"], cm[2], S_comm["col"], cm[3],
+                S_comm["ts_col"]]
+    c = out["batch_challenge"]
+    return DlogGroup(curve).vartime_multiscalar_mul(fields.pack(fid, [pow(c, i, p) for i in range(len(comm_vec))]),
+                                                    b"".join(_affine_bytes(curve, P) for P in comm_vec))
+
+
 def prove(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: dict, vk_digest: int, transcript,
           timings: dict | None = None, device_transcript: bool = False, ee: str = "hyperkzg",
           S_comm: dict | None = None):
@@ -733,31 +784,39 @@ def prove(curve, ck: CommitmentKey, S: dict, spark: SparkRepr, U: dict, W: dict,
                        is only an input of EE::prove for the HyperKZG prover, which does not use it: the caller /
                        verifier forms it from the 15 commitments.)
       ee = "mercury":  mercury.rs:891-1268, which absorbs the batched commitment: `S_comm` must hold the seven
-                       shape commitments (R1CSShapeSparkCommitment: val_A, val_B, val_C, row, col, ts_row, ts_col)."""
-    if ee not in ("hyperkzg", "mercury"):
+                       shape commitments (R1CSShapeSparkCommitment: val_A, val_B, val_C, row, col, ts_row, ts_col,
+                       as `setup` returns them).
+      ee = "ipa":      ipa_pc.rs:64-77, 174-285 -> eval_arg = (L_vec, R_vec, a_hat); absorbs the batched commitment
+                       too, so it needs `S_comm`.  `ck` must carry the generator ck_c as its blinding base and at
+                       least N bases.
+    With `timings`, ee = "ipa" adds the phases "ipa_batch_commitment", "ipa_b_vec", "ipa_inner_products",
+    "ipa_commit" and "ipa_fold" (ipa.InnerProductArgument.prove)."""
+    if ee not in ("hyperkzg", "mercury", "ipa"):
         raise ValueError(f"unknown evaluation engine {ee!r}")
-    if ee == "mercury" and S_comm is None:
-        raise ValueError("the Mercury evaluation argument needs the shape commitments S_comm")
+    if ee != "hyperkzg" and S_comm is None:
+        raise ValueError(f"the {ee} evaluation argument needs the shape commitments S_comm")
+    if ee == "ipa" and (not ck.has_h or len(ck) < spark.N):
+        raise ValueError(f"the IPA needs a key with the generator ck_c and at least N = {spark.N} bases")
     out = prove_core(curve, ck, S, spark, U, W, vk_digest, transcript, timings, device_transcript)
     if ee == "hyperkzg":
         from .spartan import hyperkzg_prove
         out["eval_arg"] = hyperkzg_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings)
         return out
-    from .mercury import mercury_prove
-    from .provider import Curve, DlogGroup
-    from .snark import _affine_bytes
+    import time
+    from .provider import Curve
     curve = Curve(curve)
-    fid = curve.scalar_field
-    p = fields.MODULUS[fid]
-    cm = out["comm_mem"]
-    comm_vec = [U["comm_W"], U["comm_E"], out["comm_L_row"], out["comm_L_col"], S_comm["val_A"], S_comm["val_B"],
-                S_comm["val_C"], cm[0], S_comm["row"], cm[1], S_comm["ts_row"], cm[2], S_comm["col"], cm[3],
-                S_comm["ts_col"]]  # ppsnark.rs comm_vec order
-    c = out["batch_challenge"]
-    C = DlogGroup(curve).vartime_multiscalar_mul(fields.pack(fid, [pow(c, i, p) for i in range(len(comm_vec))]),
-                                                 b"".join(_affine_bytes(curve, P) for P in comm_vec))
-    out["eval_arg"] = mercury_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings,
-                                    comm=C, eval_=out["batched_eval"])
+    t0 = time.perf_counter()
+    C = _batched_commitment(curve, U, S_comm, out)
+    if ee == "mercury":
+        from .mercury import mercury_prove
+        out["eval_arg"] = mercury_prove(curve, ck, out["batched_poly"], out["r_inner_batched"], transcript, timings,
+                                        comm=C, eval_=out["batched_eval"])
+        return out
+    if timings is not None:
+        timings["ipa_batch_commitment"] = timings.get("ipa_batch_commitment", 0.0) + time.perf_counter() - t0
+    from .ipa import prove_at_point
+    out["eval_arg"] = prove_at_point(curve, ck, C, out["r_inner_batched"], out["batched_eval"], out["batched_poly"],
+                                     transcript, timings)
     return out
 
 

@@ -147,14 +147,9 @@ def prove(curve, ck: CommitmentKey, S: dict, U: dict, W: dict, vk_digest: int, t
         proof["eval_arg"] = mercury_prove(curve, ck, proof["batched_poly"], proof["batched_x"], transcript, timings,
                                           comm=proof["batched_c"], eval_=proof["batched_e"])
     elif ee == "ipa":
-        from .ipa import InnerProductArgument
-        fid = Curve(curve).scalar_field
-        x = proof["batched_x"]
-        b_vec = DeviceVec(32 << len(x))  # EqPolynomial::new(point).evals(), ipa_pc.rs:73
-        x_dev = DeviceVec.from_bytes(fields.pack(fid, x))
-        check(lib().b200_eq_table_dev(fid, x_dev.ptr, len(x), b_vec.ptr, None))
-        proof["eval_arg"] = InnerProductArgument.prove(curve, ck, proof["batched_c"], b_vec, proof["batched_e"],
-                                                       proof["batched_poly"], transcript)
+        from .ipa import prove_at_point
+        proof["eval_arg"] = prove_at_point(curve, ck, proof["batched_c"], proof["batched_x"], proof["batched_e"],
+                                           proof["batched_poly"], transcript)
     else:
         raise ValueError(f"unknown evaluation engine {ee!r}")
     return proof

@@ -71,7 +71,7 @@ class SparseMatrix:
     """CSR `SparseMatrix{data, indices, indptr, cols}` (sparse.rs:235-247), device resident."""
 
     def __init__(self, fid: int, data: bytes, indices, indptr, cols: int):
-        self.fid, self.rows, self.cols = fid, len(indptr) - 1, cols
+        self.fid, self.rows, self.cols, self.nnz = fid, len(indptr) - 1, cols, int(indptr[-1])
         ia = (c_u64 * max(len(indices), 1))(*indices)
         ip = (c_u64 * len(indptr))(*indptr)
         h = c_u64(0)
