@@ -47,8 +47,9 @@ enum {
   B200_E_RANGE = 5,    /* slice outside the registered key (pedersen.rs:264 assert) */
   B200_E_ZERO = 6,     /* batch_invert met a zero (NovaError::InternalError, spartan/mod.rs:98-100) */
   B200_E_PEER = 8,     /* a peer GPU never delivered its partial sum to the exchange buffer (multi-GPU MSM) */
-  B200_E_POINT = 7     /* a key point is non-canonical or off the curve (NovaError::InvalidCommitmentKey,
+  B200_E_POINT = 7,    /* a key point is non-canonical or off the curve (NovaError::InvalidCommitmentKey,
                           hyperkzg.rs:113-119; PtauFileError::PointNotOnCurve, ptau.rs:386-388) */
+  B200_E_INDEX = 9     /* an address outside the derived table (NovaError::InvalidIndex, b200_ck_derive_by_address) */
 };
 
 /* ---- library / device ------------------------------------------------------------------ */
@@ -107,6 +108,32 @@ int b200_ck_setup_tau(int curve_id, const void* generator_affine_mont, const voi
  * what `CommitmentKey::ck()` (traits.rs / hyperkzg.rs:98-110) gives a Rust caller.  The tests hand a
  * device-generated key to the CPU oracle with it. */
 int b200_ck_export_bases(uint64_t ck_handle, size_t offset, size_t n, void* out_host);
+/* ck_derive_by_address (traits/commitment.rs:177-194, pedersen.rs:360-382, hyperkzg.rs:731-749):
+ *   derived[j] = sum_{i < m, addresses[i] = j} ck[i],  j < table_size   (a slot no address points to: the identity)
+ * so that Comm(T[addresses], ck[..m]) = Comm(T, derived) for a lookup table T: a prover holding the derived key commits
+ * to the table-sized vector in place of the lookup-sized one.  The derivation runs on the device (the bucket stage of a
+ * one-window MSM whose scalars are all 1, with the address as the bucket) and the result is a new, independent resident
+ * key of table_size bases, with its window tables built as b200_ck_register builds them (window_bits = 0 picks c from
+ * table_size; a key of 2^22 bases or more also gets its 17-bit table set).  It carries the source key's h when the
+ * source has one (HyperKZG's tau_H stays with the caller).  The call returns once the key is built; the source key may
+ * be released right after, and other calls may use the source key meanwhile.
+ * Errors, in the reference's order (nothing is registered and *out_handle is untouched on any of them; *first_bad,
+ * when given, is SIZE_MAX unless noted):
+ *   B200_E_HANDLE  unknown ck_handle
+ *   B200_E_POINT   an identity generator anywhere in ck[0 .. n), *first_bad = its index (the reference panics:
+ *                  ck_to_group_elements)
+ *   B200_E_RANGE   m > n (NovaError::InvalidCommitmentKeyLength; a prefix m < n is allowed)
+ *   B200_E_INDEX   an address >= table_size (NovaError::InvalidIndex), *first_bad = the smallest such position
+ *   B200_E_ARG     table_size = 0 (the reference returns an empty key for m = 0; a key of no bases cannot be
+ *                  registered here, as in b200_ck_register)
+ *   B200_E_RANGE   table_size too large for the 31-bit table indices (the limit of b200_ck_register)
+ * Null pointers and a window_bits outside {0} u [2, 24] give B200_E_ARG before any of these.  The host form checks the
+ * 64-bit addresses before it narrows them: an address of 2^32 + 3 is reported at its position, never taken as slot 3.
+ * Builds with -DNOVA_MSM_ARITH29 (table 0 not in the boundary format) return B200_E_ARG. */
+int b200_ck_derive_by_address_dev(uint64_t ck_handle, const uint32_t* d_addresses, size_t m, size_t table_size,
+                                  int window_bits, uint64_t* out_handle, size_t* first_bad_or_null, void* stream);
+int b200_ck_derive_by_address(uint64_t ck_handle, const uint64_t* addresses, size_t m, size_t table_size,
+                              int window_bits, uint64_t* out_handle, size_t* first_bad_or_null);
 int b200_ck_release(uint64_t ck_handle);
 int b200_ck_len(uint64_t ck_handle, size_t* n, int* window_bits, int* num_tables);
 

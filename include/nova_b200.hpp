@@ -72,6 +72,21 @@ class CommitmentKey {
     if (rc == B200_E_POINT) throw InvalidCommitmentKey(bad);
     check(rc, "b200_ck_register_checked");
   }
+  // ck_derive_by_address (traits/commitment.rs:177-194): an address outside the table (NovaError::InvalidIndex, with
+  // the smallest offending position) and more addresses than bases (NovaError::InvalidCommitmentKeyLength)
+  struct InvalidIndex : std::runtime_error {
+    size_t position;
+    explicit InvalidIndex(size_t i)
+        : std::runtime_error("InvalidIndex: address at position " + std::to_string(i) + " is outside the table"),
+          position(i) {}
+  };
+  struct InvalidCommitmentKeyLength : std::runtime_error {
+    InvalidCommitmentKeyLength() : std::runtime_error("InvalidCommitmentKeyLength: more addresses than bases") {}
+  };
+  // takes ownership of a key the library has already registered (b200_ck_derive_by_address) of n bases
+  struct Adopt {};
+  CommitmentKey(Adopt, uint64_t handle, size_t n) : handle_(handle), n_(n) {}
+  CommitmentKey(CommitmentKey&& o) noexcept : handle_(o.handle_), n_(o.n_) { o.handle_ = 0; }
   CommitmentKey(const CommitmentKey&) = delete;
   CommitmentKey& operator=(const CommitmentKey&) = delete;
   ~CommitmentKey() { if (handle_) b200_ck_release(handle_); }
@@ -136,6 +151,25 @@ struct CommitmentEngine {
   }
   static std::vector<Point> batch_commit(const CommitmentKey<C>& ck, const std::vector<std::vector<Scalar>>& vs) {
     return DlogGroup<C>::batch_vartime_multiscalar_mul(vs, ck);
+  }
+  // ck_derive_by_address (traits/commitment.rs:177-194, pedersen.rs:360-382, hyperkzg.rs:731-749), on the device:
+  // derived[j] = sum of ck[i] over the i with addresses[i] = j, j < table_size, so that
+  // commit(derived, T) == commit(ck, T[addresses]).  The new key carries ck's h and outlives ck.  An identity
+  // generator in ck (the reference's panic) throws std::logic_error; table_size = 0 throws std::logic_error too (the
+  // reference returns an empty key for no addresses; a key of no bases cannot be registered).
+  static CommitmentKey<C> ck_derive_by_address(const CommitmentKey<C>& ck, const std::vector<size_t>& addresses,
+                                               size_t table_size, int window_bits = 0) {
+    using Key = CommitmentKey<C>;
+    std::vector<uint64_t> a(addresses.begin(), addresses.end());
+    uint64_t h = 0;
+    size_t bad = SIZE_MAX;
+    int rc = b200_ck_derive_by_address(ck.handle(), a.data(), a.size(), table_size, window_bits, &h, &bad);
+    if (rc == B200_E_INDEX) throw typename Key::InvalidIndex(bad);
+    if (rc == B200_E_RANGE && a.size() > ck.len()) throw typename Key::InvalidCommitmentKeyLength();
+    if (rc == B200_E_POINT)
+      throw std::logic_error("ck_derive_by_address: generator " + std::to_string(bad) + " is the identity");
+    check(rc, "b200_ck_derive_by_address");
+    return Key(typename Key::Adopt{}, h, table_size);
   }
 };
 

@@ -867,6 +867,128 @@ int b200_ck_export_bases(uint64_t handle, size_t offset, size_t n, void* out_hos
 #endif
 }
 
+// ck_derive_by_address: reads only the source's table 0 and its h slot, through the shared_ptr (a concurrent release
+// is safe) and without the source's workspace or mutex; every temporary comes from the stream-ordered pool, sized by m
+// and table_size.
+int b200_ck_derive_by_address_dev(uint64_t ck_handle, const uint32_t* d_addresses, size_t m, size_t table_size,
+                                  int window_bits, uint64_t* out_handle, size_t* first_bad, void* stream) {
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (!out_handle || (m && !d_addresses)) return fail(B200_E_ARG, "null pointer");
+  if (window_bits != 0 && (window_bits < 2 || window_bits > 24))
+    return fail(B200_E_ARG, "window_bits %d out of range [2,24]", window_bits);
+  if (first_bad) *first_bad = SIZE_MAX;
+  auto src = get_ck(ck_handle);
+  if (!src) return fail(B200_E_HANDLE, "unknown key handle %llu", (unsigned long long)ck_handle);
+#if defined(NOVA_MSM_ARITH29)
+  return fail(B200_E_ARG, "b200_ck_derive_by_address: table 0 is not in the boundary format in this build");
+#else
+  const cudaStream_t s = pick_stream(stream);
+  const field_ops* bops = ops_for_field(CURVES[src->curve].base_fid);
+  // identity generators and out-of-range addresses in one pass; one read-back, together with h
+  dev_buf flags(s);
+  if ((rc = flags.alloc(8))) return rc;
+  CU(cudaMemsetAsync(flags.p, 0xFF, 8, s));
+  bops->derive_check(s, src->tables, src->n, d_addresses, m <= src->n ? m : 0, table_size, (uint32_t*)flags.p);
+  count_launch(1);
+  CU(cudaGetLastError());
+  uint32_t bad[2];
+  std::vector<char> h(64);
+  CU(cudaMemcpyAsync(bad, flags.p, 8, cudaMemcpyDeviceToHost, s));
+  if (src->has_h) CU(cudaMemcpyAsync(h.data(), (const char*)src->tables + src->n * 64, 64, cudaMemcpyDeviceToHost, s));
+  CU(cudaStreamSynchronize(s));
+  if (bad[0] != 0xFFFFFFFFu) {
+    if (first_bad) *first_bad = bad[0];
+    return fail(B200_E_POINT, "generator %u of the key is the identity", bad[0]);
+  }
+  if (m > src->n)
+    return fail(B200_E_RANGE, "InvalidCommitmentKeyLength: %zu addresses, key has %zu bases", m, src->n);
+  if (bad[1] != 0xFFFFFFFFu) {
+    if (first_bad) *first_bad = bad[1];
+    return fail(B200_E_INDEX, "InvalidIndex: address at position %u is outside the table of %zu", bad[1], table_size);
+  }
+  if (table_size == 0) return fail(B200_E_ARG, "table_size = 0: a key of no bases cannot be registered");
+  const int c = window_bits ? window_bits : choose_window(table_size);
+  const size_t ntables = (size_t)(FIELD_BITS[CURVES[src->curve].scalar_fid] + c - 1) / c;
+  if (table_size >= ((size_t)1 << 31) || ntables * (table_size + (src->has_h ? 1 : 0)) >= ((size_t)1 << 31))
+    return fail(B200_E_RANGE, "table of %zu bases too large for 31-bit table indices (%zu tables)", table_size, ntables);
+
+  const uint32_t K = (uint32_t)table_size;
+  dev_buf bases(s);
+  if ((rc = bases.alloc((size_t)K * 64))) return rc;
+  if (m == 0) {
+    CU(cudaMemsetAsync(bases.p, 0, (size_t)K * 64, s));
+  } else {
+    // a one-window MSM plan over m entries and K buckets; no digits and no reduction
+    msm_plan p{};
+    p.n = m;
+    p.n_ck = src->stride;
+    p.blind_i = SIZE_MAX;
+    p.h_index = src->n;
+    p.W = p.G = 1;
+    p.B = K;
+    p.L = segment_len(m);
+    p.m = 1;
+    const size_t nseg = (m + p.L - 1) / p.L;
+    p.heavy_min = HEAVY_PARTS * (uint32_t)p.L;
+    p.heavy_cap = (uint32_t)(nseg / HEAVY_PARTS + 2);
+    p.sp = make_sort_plan(K);
+    p.sort_tag = 1;  // fresh look-back words
+    const size_t look_bytes = (m + SORT_TILE - 1) / SORT_TILE * SORT_BINS * sizeof(unsigned long long);
+    dev_buf ctl(s), look(s), start(s), ent(s), ent_tmp(s), buckets(s), parts(s), pkeys(s), heavy(s), hparts(s);
+    if ((rc = ctl.alloc(SORT_CTL_WORDS * 4)) || (rc = look.alloc(look_bytes)) || (rc = start.alloc(((size_t)K + 1) * 4)) ||
+        (rc = ent.alloc(m * 8)) || (rc = ent_tmp.alloc(m * 8)) || (rc = buckets.alloc((size_t)K * XYZZ_BYTES)) ||
+        (rc = parts.alloc(2 * nseg * XYZZ_BYTES)) || (rc = pkeys.alloc(2 * nseg * 4)) ||
+        (rc = heavy.alloc(((size_t)p.heavy_cap + 1) * 4)) || (rc = hparts.alloc((size_t)p.heavy_cap * HEAVY_SPLIT * XYZZ_BYTES)))
+      return rc;
+    CU(cudaMemsetAsync(ctl.p, 0, SORT_CTL_WORDS * 4, s));
+    CU(cudaMemsetAsync(look.p, 0, look_bytes, s));
+    CU(cudaMemsetAsync(heavy.p, 0, 4, s));
+    p.sortctl = (uint32_t*)ctl.p;
+    p.look = (unsigned long long*)look.p;
+    p.start = (uint32_t*)start.p;
+    p.entries = (uint64_t*)ent.p;
+    p.entries_tmp = (uint64_t*)ent_tmp.p;
+    p.buckets = buckets.p;
+    p.parts = parts.p;
+    p.pkeys = (uint32_t*)pkeys.p;
+    p.heavy = (uint32_t*)heavy.p;
+    p.hparts = hparts.p;
+    const int sort_launches = derive_sort(s, d_addresses, p);
+    bops->accumulate(s, src->tables, p);  // every sign positive: the sum of the bases of each address
+    bops->fixup(s, p);
+    bops->derive_affine(s, p.start, K, p.buckets, bases.p);
+    count_launch(sort_launches + 1 + STAGE_KERNELS[ST_FIXUP] + 1);
+    CU(cudaGetLastError());
+  }
+  std::shared_ptr<ck_ctx> ck;
+  rc = register_key(src->curve, bases.p, true, K, src->has_h ? h.data() : nullptr, window_bits, true, ck, nullptr, s);
+  if (rc) return rc;
+  std::lock_guard<std::mutex> lk(g_handles_mu);
+  *out_handle = g_next_handle++;
+  g_handles[*out_handle] = ck;
+  return B200_OK;
+#endif
+}
+
+int b200_ck_derive_by_address(uint64_t ck_handle, const uint64_t* addresses, size_t m, size_t table_size,
+                              int window_bits, uint64_t* out_handle, size_t* first_bad) {
+  int rc = ensure_init();
+  if (rc) return rc;
+  if (m && !addresses) return fail(B200_E_ARG, "null pointer");
+  // The device form takes u32 addresses.  An address at or past table_size becomes 0xFFFFFFFF, which is past every
+  // table size the device form is given (a table of 2^32 - 1 bases fails the 31-bit limit anyway), so it is reported
+  // at its own position and never wraps onto a slot; an in-range address of 2^32 or more (only possible when the
+  // table is too large to register) is clamped below that.
+  const size_t ts = std::min(table_size, (size_t)0xFFFFFFFFu);
+  std::vector<uint32_t> a32(m);
+  for (size_t i = 0; i < m; i++)
+    a32[i] = addresses[i] >= table_size ? 0xFFFFFFFFu : (uint32_t)std::min<uint64_t>(addresses[i], 0xFFFFFFFEu);
+  return via_device({up(a32.data(), m * 4)}, [&](void** d, cudaStream_t s) {
+    return b200_ck_derive_by_address_dev(ck_handle, (const uint32_t*)d[0], m, ts, window_bits, out_handle, first_bad, s);
+  });
+}
+
 int b200_ck_release(uint64_t handle) {
   std::shared_ptr<ck_ctx> ck;
   {

@@ -1153,4 +1153,48 @@ __global__ void __launch_bounds__(256) k_on_curve(const void* __restrict__ pts, 
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// ck_derive_by_address (traits/commitment.rs:177-194, pedersen.rs:360-382, hyperkzg.rs:731-749):
+//   derived[j] = sum_{i < m, addr[i] = j} ck[i]
+// is the bucket stage of a one-window MSM whose scalars are all 1, with the address as the bucket:
+// k_address_entries (msm_sort.cuh), the radix passes, k_sort_starts, k_accumulate over the source's
+// table 0 and the fix-up kernels, then k_derive_affine in place of the reduction.
+// ------------------------------------------------------------------------------------------
+// The checks of one derivation in one pass: flags[0] = smallest index of an identity generator among the n bases of
+// table 0 (ck_to_group_elements' assertion), flags[1] = smallest position i < m of an address >= table_size
+// (NovaError::InvalidIndex).  The caller presets both to 0xFFFFFFFF and passes m <= n.  64 + 4 B read per base.
+template <class F>
+__global__ void __launch_bounds__(256) k_derive_check(const void* __restrict__ tables, size_t n,
+                                                      const uint32_t* __restrict__ addr, size_t m,
+                                                      size_t table_size, uint32_t* __restrict__ flags) {
+  using PA = msm_arith<F>;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    if (PA::aff_is_identity(PA::load_table(tables, i))) atomicMin(&flags[0], (uint32_t)i);
+    if (i < m && addr[i] >= table_size) atomicMin(&flags[1], (uint32_t)i);
+  }
+}
+
+// bucket k -> derived base k in the BOUNDARY format (affine Montgomery, identity (0,0)), the layout register_key
+// takes: a slot no address points to, or whose sum is the identity (P + (-P)), is (0,0).  One inversion per slot;
+// 128 B read and 64 B written.
+template <class F>
+__global__ void __launch_bounds__(128) k_derive_affine(const uint32_t* __restrict__ start, uint32_t K,
+                                                       const void* __restrict__ buckets, void* __restrict__ out) {
+  using PA = msm_arith<F>;
+  const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  fe_t x = fe_zero<F>(), y = fe_zero<F>();
+  if (start[k + 1] > start[k]) {  // an empty bucket holds stale data
+    fe_t X, Y, Z;
+    PA::to_jacobian_std(PA::load(buckets, k), X, Y, Z);
+    if (!fe_is_zero(Z)) {
+      const fe_t zi = fe_inv<F>(Z), zi2 = fe_sqr<F>(zi);
+      x = fe_mul<F>(X, zi2);
+      y = fe_mul<F>(Y, fe_mul<F>(zi2, zi));
+    }
+  }
+  fe_store(out, 2 * (size_t)k, x);
+  fe_store(out, 2 * (size_t)k + 1, y);
+}
+
 }  // namespace nova

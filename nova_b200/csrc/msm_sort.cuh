@@ -155,6 +155,25 @@ static __global__ void __launch_bounds__(256) k_digits_small(const void* __restr
   sort_hist_flush(s_hist, hist, sp);
 }
 
+// The address stage of ck_derive_by_address (traits/commitment.rs:177-194), in place of the digit stage: a one-window
+// MSM whose scalars are all 1 and whose bucket is the address.  Entry i = (key addr[i], sign 0, table index i), written
+// in index order, and the radix histograms of the keys.  Every radix pass then reads entries (k_sort_pass<false>), so
+// the order inside a bucket is the index order.  The caller has checked addr[i] < K <= 2^31 (no key is NO_KEY).
+static __global__ void __launch_bounds__(256) k_address_entries(const uint32_t* __restrict__ addr, size_t m,
+                                                                uint64_t* __restrict__ entries,
+                                                                uint32_t* __restrict__ hist, const sort_plan sp) {
+  __shared__ uint32_t s_hist[SORT_PASSES_MAX * SORT_BINS];
+  sort_hist_clear(s_hist);
+  for (size_t blk = (size_t)blockIdx.x * blockDim.x; blk < m; blk += (size_t)gridDim.x * blockDim.x) {
+    const size_t i = blk + threadIdx.x;
+    const bool live = i < m;  // no early exit: the whole warp takes part in sort_hist_count
+    const uint32_t key = live ? addr[i] : NO_KEY;
+    if (live) entries[i] = ((uint64_t)key << 32) | (uint32_t)i;
+    sort_hist_count(s_hist, key, sp);
+  }
+  sort_hist_flush(s_hist, hist, sp);
+}
+
 // exclusive scan over the SORT_THREADS threads of a block; *total = sum of all v.  s_tmp: SORT_WARPS words.
 NOVA_D uint32_t sort_block_scan(uint32_t v, uint32_t* s_tmp, uint32_t* total) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

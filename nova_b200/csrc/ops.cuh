@@ -129,6 +129,11 @@ struct field_ops {
   // R1CSShapeSparkRepr::new (k_spark_repr): row, col, ts_row, ts_col (Montgomery) and the u32 row / col indices
   void (*spark_repr)(cudaStream_t, const spark_mats&, size_t N, void* row, void* col, void* ts_row, void* ts_col,
                      uint32_t* row_idx, uint32_t* col_idx);
+  // ck_derive_by_address (msm_kernels.cuh): flags[0] = first identity base of table 0, flags[1] = first address
+  // >= table_size among addr[0 .. m), m <= n (caller presets 0xFFFFFFFF); buckets [0, K) -> boundary-format bases
+  void (*derive_check)(cudaStream_t, const void* tables, size_t n, const uint32_t* addr, size_t m, size_t table_size,
+                       uint32_t* flags);
+  void (*derive_affine)(cudaStream_t, const uint32_t* start, uint32_t K, const void* buckets, void* out_bases);
 };
 // SM count of the H100 SXM (sm_90a): grids below are sized in whole waves of it
 constexpr int NUM_SMS = 132;
@@ -176,5 +181,8 @@ inline const field_ops* ops_for_field(int fid) {
 // field-independent MSM stages (msm_common.cu)
 int msm_sort(cudaStream_t, const msm_plan&);  // returns the number of kernels launched
 void msm_digits_small(cudaStream_t, const void* scalars, int elem_bytes, const msm_plan&);
+// ck_derive_by_address: the address stage (k_address_entries) and the radix passes over p.n = m entries, then the
+// starts of the p.B buckets; returns the number of kernels launched
+int derive_sort(cudaStream_t, const uint32_t* addr, const msm_plan&);
 
 }  // namespace nova

@@ -490,6 +490,13 @@ struct ops_impl {
     k_red_final_q<F><<<1, 384, 0, s>>>(nullptr, 0, 4, 4, out_jac, p.peer);  // G = 0: the local partial is the identity
 #endif
   }
+  static void derive_check(cudaStream_t s, const void* tables, size_t n, const uint32_t* addr, size_t m,
+                           size_t table_size, uint32_t* flags) {
+    if (n) k_derive_check<F><<<stream_grid(n, 256), 256, 0, s>>>(tables, n, addr, m, table_size, flags);
+  }
+  static void derive_affine(cudaStream_t s, const uint32_t* start, uint32_t K, const void* buckets, void* out) {
+    if (K) k_derive_affine<F><<<(unsigned)((K + 127) / 128), 128, 0, s>>>(start, K, buckets, out);
+  }
   static constexpr field_ops table() {
     return field_ops{F::ID,  digits,       expand_key, accumulate, fixup,   reduce,
                      sum_points, jacobian_sum, index_bases, cross_term, axpy,       vec_add, bind_top, bind_top_multi, vec_mul, logup_hash,
@@ -499,7 +506,7 @@ struct ops_impl {
                      powers_canonical, scalar_bases, poseidon_ro, to_mont, exchange_identity,
                      sc_round_batched_fused, sc_reduce_multi_partials, gather_heads, poly_eval_small_multi,
                      eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly,
-                     neutron_evals, pow_split_evals, lerp, spark_repr};
+                     neutron_evals, pow_split_evals, lerp, spark_repr, derive_check, derive_affine};
   }
 };
 

@@ -10,10 +10,19 @@ _LIB = None
 c_size_t, c_int, c_void_p, c_u64 = ctypes.c_size_t, ctypes.c_int, ctypes.c_void_p, ctypes.c_uint64
 
 
+# status codes of include/nova_b200.h
+B200_OK, B200_E_ARG, B200_E_CUDA, B200_E_HANDLE, B200_E_NOMEM, B200_E_RANGE = 0, 1, 2, 3, 4, 5
+B200_E_ZERO, B200_E_POINT, B200_E_PEER, B200_E_INDEX = 6, 7, 8, 9
+ERROR_NAMES = {B200_E_ARG: "B200_E_ARG", B200_E_CUDA: "B200_E_CUDA", B200_E_HANDLE: "B200_E_HANDLE",
+               B200_E_NOMEM: "B200_E_NOMEM", B200_E_RANGE: "B200_E_RANGE", B200_E_ZERO: "B200_E_ZERO",
+               B200_E_POINT: "B200_E_POINT", B200_E_PEER: "B200_E_PEER", B200_E_INDEX: "B200_E_INDEX"}
+
+
 class B200Error(RuntimeError):
     def __init__(self, code: int, msg: str):
         super().__init__(f"nova_b200 error {code}: {msg}")
         self.code = code
+        self.name = ERROR_NAMES.get(code, "unknown")
 
 
 def library_path() -> str:
@@ -63,6 +72,10 @@ SIGNATURES = {
     "b200_msm_sharded_dev": [c_u64, c_size_t, _P, c_size_t, c_u64, _P, _P],
     "b200_ck_setup_tau": [c_int, _P, _P, c_size_t, c_int, ctypes.POINTER(c_u64)],
     "b200_ck_export_bases": [c_u64, c_size_t, c_size_t, _P],
+    "b200_ck_derive_by_address": [c_u64, ctypes.POINTER(c_u64), c_size_t, c_size_t, c_int, ctypes.POINTER(c_u64),
+                                  ctypes.POINTER(c_size_t)],
+    "b200_ck_derive_by_address_dev": [c_u64, _P, c_size_t, c_size_t, c_int, ctypes.POINTER(c_u64),
+                                      ctypes.POINTER(c_size_t), _P],
     "b200_ck_release": [c_u64],
     "b200_ck_len": [c_u64, ctypes.POINTER(c_size_t), ctypes.POINTER(c_int), ctypes.POINTER(c_int)],
     "b200_msm": [c_u64, c_size_t, _P, c_size_t, _P],

@@ -22,7 +22,7 @@ import ctypes
 import enum
 
 from . import fields
-from .native import c_size_t, c_u64, check, lib
+from .native import B200Error, c_size_t, c_u64, check, lib
 
 
 class Curve(enum.IntEnum):
@@ -254,6 +254,33 @@ class CommitmentEngine:
         assert hi <= len(ck) and hi <= len(v)
         P = self.group.vartime_multiscalar_mul_small(v[lo:hi], ck, elem_bytes, max_num_bits, base_offset=lo)
         return self._plus_blind(ck, P, r)
+
+    def ck_derive_by_address(self, ck: CommitmentKey, addresses, table_size: int, window_bits: int = 0) -> CommitmentKey:
+        """traits/commitment.rs:177-194 (pedersen.rs:360-382, hyperkzg.rs:731-749): the key of table_size bases with
+        derived[j] = sum of ck[i] over the i < len(addresses) with addresses[i] = j, built on the device.  Then
+        commit(derived, T) == commit(ck, T[addresses]).  The new key has no host copy of its bases; its h is ck's.
+        Errors raise B200Error with .code (B200_E_POINT, B200_E_RANGE, B200_E_INDEX, ...) and .first_bad."""
+        m = len(addresses)
+        arr = (c_u64 * max(m, 1))(*addresses)
+        return self._derived(ck, lambda out, bad: lib().b200_ck_derive_by_address(
+            ck.handle, arr, m, table_size, window_bits, out, bad), table_size)
+
+    def ck_derive_by_address_dev(self, ck: CommitmentKey, d_addresses, m: int, table_size: int, window_bits: int = 0,
+                                 stream=None) -> CommitmentKey:
+        """The same from m u32 addresses in device memory (a device pointer), on `stream` (None: the library's)."""
+        return self._derived(ck, lambda out, bad: lib().b200_ck_derive_by_address_dev(
+            ck.handle, d_addresses, m, table_size, window_bits, out, bad, stream), table_size)
+
+    def _derived(self, ck: CommitmentKey, call, table_size: int) -> CommitmentKey:
+        out, bad = c_u64(0), c_size_t(-1)
+        rc = call(ctypes.byref(out), ctypes.byref(bad))
+        if rc:
+            err = B200Error(rc, lib().b200_last_error().decode())
+            err.first_bad = None if bad.value == ctypes.c_size_t(-1).value else bad.value
+            raise err
+        key = CommitmentKey.from_handle(self.curve, out.value, None, ck.h, table_size)
+        key.has_h = ck.has_h
+        return key
 
     def commit_sparse(self, ck: CommitmentKey, indices, scalars: bytes, r: bytes | None = None):
         """pedersen.rs:411-427: gather ck[indices] on the host, one MSM over the gathered bases (+ h * r as
