@@ -535,6 +535,15 @@ int b200_ipa_scalars_dev(int field_id, const void* a, const void* w, size_t n, s
 /* nk == 0: w := 1 ; else w[j] *= (j & nk/2) ? r : r_inv */
 int b200_ipa_weights_dev(int field_id, void* w, size_t n, size_t nk, const void* r, const void* r_inv,
                          void* stream);
+/* The verifier's tensor vector s of InnerProductArgument::verify (ipa_pc.rs:334-349), times a scale:
+ *     out[i] = scale * prod_{j < L} (bit j of i, most significant first ? r[j] : r_inv[j]),   i < 2^L
+ * (the reference's s[0] = prod r^-1, s[i] = s[i - 2^pos] * r^2[L-1-pos] is the same product).  r, r_inv: L
+ * Montgomery elements each; d_scale_or_null: one element, or NULL for 1.  It is also the prover's weights w after
+ * all L rounds of b200_ipa_weights_dev.  With scale = a_hat and the key registered with h = ck_c, the verifier's
+ * a_hat * ck_hat + a_hat * b_hat * (r0 * ck_c) is one b200_commit_dev(key, out, 2^L, blind = a_hat * b_hat * r0).
+ * B200_E_ARG for L outside 0 .. 31 or a null pointer; nothing is written then. */
+int b200_ipa_s_dev(int field_id, const void* d_r, const void* d_r_inv, int L, const void* d_scale_or_null, void* d_out,
+                   void* stream);
 
 /* ---- sparse matrices (r1cs/sparse.rs:19-319) ------------------------------------------------
  * CSR as in SparseMatrix{data, indices, indptr, cols} (sparse.rs:235-247); registration uploads
@@ -560,6 +569,20 @@ int b200_gather_dev(const void* d_table, const uint32_t* d_idx, size_t n, void* 
  * small: B200_E_RANGE.  Nothing is written on an error. */
 int b200_spark_repr_dev(uint64_t hA, uint64_t hB, uint64_t hC, size_t N, void* const* d_vecs, uint32_t* d_row_idx,
                         uint32_t* d_col_idx, void* stream);
+/* The verifier's matrix evaluations, multi_evaluate of RelaxedR1CSSNARK::verify (spartan/snark.rs:325-355):
+ *     out[y] = sum over the entries (row, col, val) of matrix y of T_x[row] * T_y[col] * val,   y < k
+ * for the k <= 3 matrices behind m_handles (a host array), in one launch (partitioned by entry ranges, so long and
+ * empty rows cost no imbalance).  d_Tx / d_Ty: tx_len / ty_len Montgomery elements; d_out: k elements.
+ *   B200_E_HANDLE  an unknown handle
+ *   B200_E_ARG     k = 0, k > 3, matrices of different fields, a null pointer
+ *   B200_E_RANGE   rows > tx_len or cols > ty_len of some matrix (the reference would index out of bounds)
+ * Checked before any launch; nothing is written on an error.  A matrix without entries gives 0. */
+int b200_r1cs_eval_dev(const uint64_t* m_handles, size_t k, const void* d_Tx, size_t tx_len, const void* d_Ty,
+                       size_t ty_len, void* d_out, void* stream);
+/* The same from the points, as the reference's closure takes them: T_x = eq(r_x) (2^ell_x entries) and
+ * T_y = eq(r_y) (2^ell_y) are built on the device; r_x, r_y, out are host Montgomery elements.  ell_x, ell_y <= 34. */
+int b200_r1cs_eval(const uint64_t* m_handles, size_t k, const void* r_x, int ell_x, const void* r_y, int ell_y,
+                   void* out);
 /* R1CSShape::multiply_vec / multiply_vec_pair (r1cs/mod.rs:407-471): k matrices, one or two z */
 int b200_spmv_multi(const uint64_t* m_handles, size_t k, const void* z1, const void* z2_or_null,
                     size_t z_len, void* const* out1, void* const* out2_or_null);

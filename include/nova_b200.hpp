@@ -11,6 +11,8 @@
 //   nova::b200::fold_witness, bind_poly_var_top                         r1cs/mod.rs:1044-1107,
 //                                                                       polys/multilinear.rs:65-84
 //   nova::b200::sumcheck_eval                                           spartan/sumcheck.rs (round sums)
+//   nova::b200::R1CSShape(Dev)::multi_evaluate, ipa_s                   spartan/snark.rs:325-355,
+//                                                                       ipa_pc.rs:334-349 (verifiers)
 //
 // Conventions: `Scalar` / `Affine` / `Point` are the FFI layouts (32 / 64 / 96 bytes).  Infallible
 // trait functions (MSM, commit) throw std::logic_error on length mismatch (the reference
@@ -205,6 +207,15 @@ struct R1CSShape {
     check(b200_spmv_multi(hs, 3, z.data(), nullptr, z.size(), o, nullptr), "b200_spmv_multi");
     return out;
   }
+  // [A(r_x, r_y), B(r_x, r_y), C(r_x, r_y)] = sum over each matrix's entries of eq(r_x)[row] eq(r_y)[col] val: the
+  // verifier's multi_evaluate (spartan/snark.rs:325-355); both eq tables are built on the device (b200_r1cs_eval)
+  std::array<Scalar, 3> multi_evaluate(const std::vector<Scalar>& r_x, const std::vector<Scalar>& r_y) const {
+    std::array<Scalar, 3> out{};
+    uint64_t hs[3] = {A.handle(), B.handle(), C.handle()};
+    check(b200_r1cs_eval(hs, 3, r_x.data(), (int)r_x.size(), r_y.data(), (int)r_y.size(), out.data()),
+          "b200_r1cs_eval");
+    return out;
+  }
   // T = AZ o BZ - u*CZ - E1 (- E2)   (commit_T / commit_T_relaxed, r1cs/mod.rs:614-620, 650-657)
   std::vector<Scalar> cross_term(const std::vector<Scalar>& az, const std::vector<Scalar>& bz,
                                  const std::vector<Scalar>& cz, const std::vector<Scalar>& e1, const Scalar& u,
@@ -293,6 +304,19 @@ inline Point commit_resident(const CommitmentKey<C>& ck, const DeviceVec& v, con
   return P;
 }
 
+// The IPA verifier's tensor vector (ipa_pc.rs:334-349) on the device: s[i] = scale * prod_j (bit j of i, most
+// significant first ? r[j] : r_inv[j]), 2^L entries for the L = r.len() round challenges (b200_ipa_s_dev).  With
+// scale = a_hat, commit_resident(ck, s, &blind) is the verifier's a_hat <s, ck> + blind * ck_c in one MSM.
+inline DeviceVec ipa_s(int field, const DeviceVec& r, const DeviceVec& r_inv, const Scalar* scale = nullptr) {
+  if (r_inv.len() != r.len()) throw std::invalid_argument("InvalidInputLength");
+  DeviceVec out((size_t)1 << r.len()), sc;
+  if (scale) sc = DeviceVec(std::vector<Scalar>{*scale});
+  check(b200_ipa_s_dev(field, r.ptr(), r_inv.ptr(), (int)r.len(), scale ? sc.ptr() : nullptr, out.ptr(), nullptr),
+        "b200_ipa_s_dev");
+  check(b200_sync(), "b200_sync");  // `sc` may now go
+  return out;
+}
+
 // CommitmentKey::new's on-curve loop (hyperkzg.rs:113-119): index of the first off-curve base, or SIZE_MAX
 template <class C>
 inline size_t validate_key(const std::vector<Affine>& ck) {
@@ -347,6 +371,17 @@ struct R1CSShapeDev {
     check(b200_sync(), "b200_sync");
     check(b200_memcpy_h2d((char*)out.ptr() + 32 * num_vars, tail.data(), 32 * tail.size()), "b200_memcpy_h2d");
     return out;
+  }
+  // multi_evaluate (spartan/snark.rs:325-355) on resident eq tables T_x (>= num_cons entries) and T_y (>= the
+  // matrices' columns): one b200_r1cs_eval_dev over A, B and C
+  std::array<Scalar, 3> multi_evaluate(const DeviceVec& T_x, const DeviceVec& T_y) const {
+    DeviceVec out(3);
+    uint64_t hs[3] = {A.handle(), B.handle(), C.handle()};
+    check(b200_r1cs_eval_dev(hs, 3, T_x.ptr(), T_x.len(), T_y.ptr(), T_y.len(), out.ptr(), nullptr),
+          "b200_r1cs_eval_dev");
+    std::array<Scalar, 3> r{};
+    check(b200_memcpy_d2h(r.data(), out.ptr(), 96), "b200_memcpy_d2h");
+    return r;
   }
   std::array<DeviceVec, 3> multiply_vec(const DeviceVec& zv) const {
     std::array<DeviceVec, 3> out{DeviceVec(num_cons), DeviceVec(num_cons), DeviceVec(num_cons)};

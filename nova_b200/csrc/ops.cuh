@@ -16,6 +16,7 @@ struct multi_args;     // poly_kernels.cuh
 struct poly_multi_args;
 struct scb_tail_args;  // sumcheck_tail.cuh
 struct spark_mats;     // poly_kernels.cuh
+struct r1cs_mats;      // poly_kernels.cuh
 
 struct field_ops {
   int field_id;
@@ -134,6 +135,13 @@ struct field_ops {
   void (*derive_check)(cudaStream_t, const void* tables, size_t n, const uint32_t* addr, size_t m, size_t table_size,
                        uint32_t* flags);
   void (*derive_affine)(cudaStream_t, const uint32_t* start, uint32_t K, const void* buckets, void* out_bases);
+  // the verifier's matrix evaluations (k_r1cs_eval + k_r1cs_final): out[y] = sum_e T_x[row_e] T_y[col_e] val_e over
+  // matrix y < k <= 3; scratch >= r1cs_eval_scratch_elems(k) * 32 B
+  void (*r1cs_eval)(cudaStream_t, const r1cs_mats&, int k, const void* tx, const void* ty, void* scratch, void* out);
+  // the IPA verifier's s (k_ipa_s_half, k_eq_outer): out[i] = scale * prod_j (bit j of i, MSB first ? r_j : r_inv_j),
+  // i < 2^L; scratch >= ipa_s_scratch_elems(L) * 32 B
+  void (*ipa_s)(cudaStream_t, const void* r, const void* r_inv, int L, const void* scale_or_null, void* scratch,
+                void* out);
 };
 // SM count of the H100 SXM (sm_90a): grids below are sized in whole waves of it
 constexpr int NUM_SMS = 132;
@@ -165,6 +173,15 @@ inline size_t neutron_evals_blocks(size_t n) {
   return g < 1 ? 1 : (g > NEUTRON_MAX_BLOCKS ? NEUTRON_MAX_BLOCKS : g);
 }
 inline size_t neutron_evals_scratch_elems(size_t n) { return 5 * neutron_evals_blocks(n); }
+// k_r1cs_eval: at least R1CS_MIN_CHUNK entries per thread, at most R1CS_EVAL_BLOCKS blocks of 256 threads per matrix
+constexpr size_t R1CS_MIN_CHUNK = 16;
+constexpr unsigned R1CS_EVAL_BLOCKS = NUM_SMS * 2;
+inline size_t r1cs_eval_scratch_elems(int k) { return (size_t)k * R1CS_EVAL_BLOCKS; }
+// k_ipa_s_half writes the whole s directly up to IPA_S_DIRECT_BITS bits; above, two half tables and their outer product
+constexpr int IPA_S_DIRECT_BITS = 10;
+inline size_t ipa_s_scratch_elems(int L) {
+  return L <= IPA_S_DIRECT_BITS ? 0 : ((size_t)1 << (L - L / 2)) + ((size_t)1 << (L / 2));
+}
 
 extern const field_ops OPS_BN254_FR, OPS_BN254_FQ, OPS_PALLAS_FP, OPS_PALLAS_FQ;
 

@@ -497,6 +497,30 @@ struct ops_impl {
   static void derive_affine(cudaStream_t s, const uint32_t* start, uint32_t K, const void* buckets, void* out) {
     if (K) k_derive_affine<F><<<(unsigned)((K + 127) / 128), 128, 0, s>>>(start, K, buckets, out);
   }
+  static void r1cs_eval(cudaStream_t s, const r1cs_mats& m, int k, const void* tx, const void* ty, void* scratch,
+                        void* out) {
+    size_t nnz = 0;
+    for (int y = 0; y < k; y++) nnz = m.nnz[y] > nnz ? m.nnz[y] : nnz;
+    const size_t want = (nnz + 256 * R1CS_MIN_CHUNK - 1) / (256 * R1CS_MIN_CHUNK);
+    const unsigned gx = (unsigned)(want < 1 ? 1 : (want > R1CS_EVAL_BLOCKS ? R1CS_EVAL_BLOCKS : want));
+    const size_t threads = (size_t)gx * 256, chunk = nnz ? (nnz + threads - 1) / threads : 1;
+    k_r1cs_eval<F><<<dim3(gx, (unsigned)k), 256, 0, s>>>(m, tx, ty, chunk, scratch);
+    k_r1cs_final<F><<<dim3(1, (unsigned)k), 256, 0, s>>>(scratch, (int)gx, out);
+  }
+  static void ipa_s(cudaStream_t s, const void* r, const void* r_inv, int L, const void* scale, void* scratch,
+                    void* out) {
+    if (L <= IPA_S_DIRECT_BITS) {
+      k_ipa_s_half<F><<<(unsigned)((((size_t)1 << L) + 255) / 256), 256, 0, s>>>(r, r_inv, L, scale, out);
+      return;
+    }
+    const int rb = L / 2, lb = L - rb;
+    void* left = scratch;
+    void* right = (char*)scratch + ((size_t)32 << lb);
+    k_ipa_s_half<F><<<(unsigned)((((size_t)1 << lb) + 255) / 256), 256, 0, s>>>(r, r_inv, lb, scale, left);
+    k_ipa_s_half<F><<<(unsigned)((((size_t)1 << rb) + 255) / 256), 256, 0, s>>>(
+        (const char*)r + 32 * lb, (const char*)r_inv + 32 * lb, rb, nullptr, right);
+    k_eq_outer<F><<<stream_grid((size_t)1 << L, 256), 256, 0, s>>>(left, right, rb, (size_t)1 << L, out);
+  }
   static constexpr field_ops table() {
     return field_ops{F::ID,  digits,       expand_key, accumulate, fixup,   reduce,
                      sum_points, jacobian_sum, index_bases, cross_term, axpy,       vec_add, bind_top, bind_top_multi, vec_mul, logup_hash,
@@ -506,7 +530,7 @@ struct ops_impl {
                      powers_canonical, scalar_bases, poseidon_ro, to_mont, exchange_identity,
                      sc_round_batched_fused, sc_reduce_multi_partials, gather_heads, poly_eval_small_multi,
                      eq_prefix_tables, sc_reduce_multi, scb_tail, mat_vec_rows, mercury_s_poly,
-                     neutron_evals, pow_split_evals, lerp, spark_repr, derive_check, derive_affine};
+                     neutron_evals, pow_split_evals, lerp, spark_repr, derive_check, derive_affine, r1cs_eval, ipa_s};
   }
 };
 

@@ -923,6 +923,107 @@ __global__ void __launch_bounds__(256) k_spark_repr(const spark_mats m, size_t N
 }
 
 // ------------------------------------------------------------------------------------------
+// The verifier's R1CS matrix evaluations (multi_evaluate, spartan/snark.rs:325-355):
+//   out[y] = sum over the entries (row, col, val) of matrix y of T_x[row] * T_y[col] * val,   y < k <= 3.
+// Work is split by ENTRY range, not by row: thread g of matrix y (grid.y) takes entries [g chunk, (g+1) chunk)
+// (and every grid's worth of slices after it, should the launch not cover nnz),
+// finds the row of its first entry by binary search in indptr (as k_spark_repr does), keeps a running row sum of
+// T_y[col] * val and multiplies it by T_x[row] only when the row ends -- one product per row boundary plus one per
+// general coefficient (codes +-1..7 cost adds, small_mul).  A long row spreads over many threads and a run of empty
+// rows is skipped by one more search, so no thread's work depends on the row lengths.  Field sums are exact, so the
+// split does not change the result.  partials[y * gridDim.x + x] feed k_r1cs_final.
+// ------------------------------------------------------------------------------------------
+constexpr int R1CS_MAX_MATS = 3;
+struct r1cs_mats {
+  const uint32_t* indptr[R1CS_MAX_MATS];
+  const uint32_t* colidx[R1CS_MAX_MATS];
+  const int8_t* codes[R1CS_MAX_MATS];
+  const void* vals[R1CS_MAX_MATS];
+  size_t rows[R1CS_MAX_MATS];
+  size_t nnz[R1CS_MAX_MATS];
+};
+
+// the row holding entry e: the largest r in [lo, rows) with ip[r] <= e (ip[lo] <= e < ip[rows] = nnz)
+NOVA_D size_t r1cs_row_of(const uint32_t* __restrict__ ip, size_t lo, size_t rows, size_t e) {
+  size_t hi = rows;
+  while (hi - lo > 1) {
+    const size_t mid = (lo + hi) / 2;
+    if (ip[mid] <= e) lo = mid;
+    else hi = mid;
+  }
+  return lo;
+}
+
+template <class F>
+__global__ void __launch_bounds__(256) k_r1cs_eval(const r1cs_mats m, const void* __restrict__ tx,
+                                                   const void* __restrict__ ty, size_t chunk,
+                                                   void* __restrict__ partials) {
+  __shared__ fe_t sm[8];
+  const int y = blockIdx.y;
+  const uint32_t* ip = m.indptr[y];
+  const uint32_t* ci = m.colidx[y];
+  const int8_t* codes = m.codes[y];
+  const void* vals = m.vals[y];
+  const size_t nnz = m.nnz[y], rows = m.rows[y];
+  fe_t acc[1] = {fe_zero<F>()};
+  const size_t stride = (size_t)gridDim.x * blockDim.x * chunk;  // one slice per thread when the launch covers nnz
+  // the entries are [ip[0], ip[rows]): registration allows an indptr that does not start at 0, and the reference
+  // (par_windows over indptr) never reads the entries before ip[0]; rows == 0 gives ip[0] == nnz, no work
+  for (size_t e0 = ip[0] + ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * chunk; e0 < nnz; e0 += stride) {
+    const size_t e1 = e0 + chunk < nnz ? e0 + chunk : nnz;
+    size_t row = r1cs_row_of(ip, 0, rows, e0);
+    size_t next = ip[row + 1];
+    fe_t s = fe_zero<F>();
+    for (size_t e = e0; e < e1; e++) {
+      if (e >= next) {  // row ends: weigh its sum, then find the row of e (the next one, or past a run of empty rows)
+        acc[0] = fe_add<F>(acc[0], fe_mul<F>(fe_load(tx, row), s));
+        s = fe_zero<F>();
+        row = ip[row + 2] > e ? row + 1 : r1cs_row_of(ip, row + 1, rows, e);
+        next = ip[row + 1];
+      }
+      const fe_t t = fe_load(ty, ci[e]);
+      const int c = codes[e];
+      s = fe_add<F>(s, c == 0 ? fe_mul<F>(fe_load(vals, e), t) : small_mul<F>(c, t));
+    }
+    acc[0] = fe_add<F>(acc[0], fe_mul<F>(fe_load(tx, row), s));
+  }
+  block_sum<F, 1>(acc, sm);
+  if (threadIdx.x == 0) fe_store(partials, (size_t)blockIdx.y * gridDim.x + blockIdx.x, acc[0]);
+}
+
+// block y: out[y] = sum of the nblocks partials of matrix y
+template <class F>
+__global__ void __launch_bounds__(256) k_r1cs_final(const void* __restrict__ partials, int nblocks,
+                                                    void* __restrict__ out) {
+  __shared__ fe_t sm[8];
+  fe_t acc[1] = {fe_zero<F>()};
+  for (int b = threadIdx.x; b < nblocks; b += blockDim.x)
+    acc[0] = fe_add<F>(acc[0], fe_load_rw(partials, (size_t)blockIdx.y * nblocks + b));
+  block_sum<F, 1>(acc, sm);
+  if (threadIdx.x == 0) fe_store(out, blockIdx.y, acc[0]);
+}
+
+// ------------------------------------------------------------------------------------------
+// The IPA verifier's tensor vector (ipa_pc.rs:334-349): s[i] = scale * prod_j (bit j of i, MSB first ? r_j : r_j^-1),
+// the reference's s[0] = prod r^-1, s[i] = s[i - 2^pos] r^2_{L-1-pos} written as one product per entry.  Built as
+// an eq table is: each half table entry is a direct product over its bits (this kernel, `scale` folded into the
+// left half only), and s is their outer product (k_eq_outer).
+// ------------------------------------------------------------------------------------------
+template <class F>
+__global__ void __launch_bounds__(256) k_ipa_s_half(const void* __restrict__ r, const void* __restrict__ r_inv,
+                                                    int bits, const void* __restrict__ scale_or_null,
+                                                    void* __restrict__ out) {
+  const size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= ((size_t)1 << bits)) return;
+  fe_t acc = scale_or_null ? fe_load(scale_or_null, 0) : fe_one<F>();
+  for (int j = 0; j < bits; j++) {
+    const bool bit = (idx >> (bits - 1 - j)) & 1;
+    acc = fe_mul<F>(acc, fe_load(bit ? r : r_inv, j));
+  }
+  fe_store(out, idx, acc);
+}
+
+// ------------------------------------------------------------------------------------------
 // NeutronNova folding prover pieces (neutron/nifs.rs, spartan/polys/power.rs)
 // ------------------------------------------------------------------------------------------
 // prove_helper (nifs.rs:29-186) before the rho factors.  Row k = i*left + j; with V_t = V1 + t (V2 - V1)

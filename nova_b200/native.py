@@ -87,6 +87,7 @@ SIGNATURES = {
     "b200_fold_halves_dev": [c_int, _P, c_size_t, _P, _P, _P, _P],
     "b200_ipa_scalars_dev": [c_int, _P, _P, c_size_t, c_size_t, _P, _P, _P],
     "b200_ipa_weights_dev": [c_int, _P, c_size_t, c_size_t, _P, _P, _P],
+    "b200_ipa_s_dev": [c_int, _P, _P, c_int, _P, _P, _P],
     "b200_msm_batch": [c_u64, ctypes.POINTER(_P), ctypes.POINTER(c_size_t), c_size_t, _P],
     "b200_msm_small": [c_u64, c_size_t, _P, c_int, c_size_t, c_int, _P],
     "b200_msm_indices": [c_u64, ctypes.POINTER(c_u64), c_size_t, _P],
@@ -154,6 +155,8 @@ SIGNATURES = {
     "b200_gather": [_P, c_size_t, ctypes.POINTER(c_u64), c_size_t, _P],
     "b200_gather_dev": [_P, _P, c_size_t, _P, _P],
     "b200_spark_repr_dev": [c_u64, c_u64, c_u64, c_size_t, ctypes.POINTER(_P), _P, _P, _P],
+    "b200_r1cs_eval_dev": [ctypes.POINTER(c_u64), c_size_t, _P, c_size_t, _P, c_size_t, _P, _P],
+    "b200_r1cs_eval": [ctypes.POINTER(c_u64), c_size_t, _P, c_int, _P, c_int, _P],
     "b200_spmv_multi": [ctypes.POINTER(c_u64), c_size_t, _P, _P, c_size_t, ctypes.POINTER(_P),
                         ctypes.POINTER(_P)],
 }

@@ -19,6 +19,11 @@ W, E and the batched opening polynomial stay resident; the caller hands the resu
 argument (spartan.hyperkzg_prove_resident).  The transcript object is passed in and advanced exactly
 as E::TE is in the reference (needs `absorb_bytes`, `squeeze` and the serialisable fields `round`,
 `state`, `buf`).
+
+verify_core / verify restate RelaxedR1CSSNARK::verify (snark.rs:259-396): the sum-check checks and the batch
+evaluation claim are O(log N) host algebra; the three R1CS matrix evaluations (multi_evaluate, snark.rs:325-355),
+the verifier's only O(nnz) step, run on the device (b200_eq_table_dev x2, b200_r1cs_eval_dev), and with the IPA
+evaluation engine so do the opening's tensor vector and its n-point commitment (ipa.InnerProductArgument.verify).
 """
 from __future__ import annotations
 
@@ -26,7 +31,7 @@ from . import fields
 from .native import check, lib
 from .ppsnark import View, _as_dev, _mle_eval, _rlc_dev, commitment_transcript_bytes, dev_scalar, dev_zeros, to_repr
 from .provider import CommitmentKey, Curve, DlogGroup, _cbuf
-from .spartan import DeviceVec, SumcheckProof
+from .spartan import DeviceVec, R1CSShape, SumcheckProof
 
 
 def _affine_bytes(curve: Curve, P) -> bytes:
@@ -153,3 +158,123 @@ def prove(curve, ck: CommitmentKey, S: dict, U: dict, W: dict, vk_digest: int, t
     else:
         raise ValueError(f"unknown evaluation engine {ee!r}")
     return proof
+
+
+def _eq_evaluate(p, a, b) -> int:
+    """EqPolynomial::evaluate (polys/eq.rs:38-47): prod (a_i b_i + (1 - a_i)(1 - b_i))"""
+    out = 1
+    for x, y in zip(a, b):
+        out = out * (x * y + (1 - x) * (1 - y)) % p
+    return out
+
+
+def _sparse_poly_evaluate(p, num_vars, Z, r) -> int:
+    """SparsePolynomial::evaluate (polys/multilinear.rs:207-225) of the public IO (u, X) at r."""
+    assert len(r) == num_vars
+    nvz = (max(len(Z), 1) - 1).bit_length()  # log2 of next_power_of_two(len(Z))
+    assert num_vars - 1 - nvz >= 0, "public IO too long for the shape"
+    k = num_vars - 1 - nvz
+    tail = r[k:]  # Z pairs with the first len(Z) entries of eq(tail), each a product over its bits
+    partial = 0
+    for i, z in enumerate(Z):
+        chi = 1
+        for j, x in enumerate(tail):
+            chi = chi * (x if (i >> (len(tail) - 1 - j)) & 1 else 1 - x) % p
+        partial += z * chi
+    common = 1
+    for x in r[:k]:
+        common = common * (1 - x) % p
+    return common * partial % p
+
+
+def verify_core(curve, S: dict, U: dict, vk_digest: int, proof: dict, transcript, timings: dict | None = None):
+    """RelaxedR1CSSNARK::verify (snark.rs:259-396) up to EE::verify, with batch_eval_verify (spartan/mod.rs:436-480):
+    re-derives every challenge, checks both sum-checks' final claims -- the inner one against the three matrix
+    evaluations, computed on the device -- and the batch-evaluation claim.  S, U, vk_digest as in prove_core; `proof`
+    the fields prove_core returns (sc_proof_outer, claims_outer, eval_E, sc_proof_inner, eval_W, sc_proof_batch,
+    evals_batch); `transcript` fresh, labelled b"RelaxedR1CSSNARK", and advanced to where EE::verify starts.
+    Returns the joint claim (C, x, e) for any evaluation engine; a failed check raises
+    ValueError("InvalidSumcheckProof").  `timings` (optional): "sumcheck_checks", "eq_tables", "matrix_eval",
+    "batch_eval_verify" in seconds."""
+    from .ipa import _marker
+    mark = _marker(timings)
+    curve = Curve(curve)
+    fid = curve.scalar_field
+    p = fields.MODULUS[fid]
+    num_cons, num_vars = S["num_cons"], S["num_vars"]
+    nrx, nry = num_cons.bit_length() - 1, num_vars.bit_length()
+    assert 1 << nrx == num_cons and 1 << (nry - 1) == num_vars and len(U["X"]) < num_vars
+    u = U["u"] % p
+    tr = transcript
+    tr.absorb_bytes(b"vk", to_repr(vk_digest % p))
+    tr.absorb_bytes(b"U", commitment_transcript_bytes(U["comm_W"]) + commitment_transcript_bytes(U["comm_E"])
+                    + to_repr(u) + b"".join(to_repr(x % p) for x in U["X"]))
+    tau = [tr.squeeze(b"t") for _ in range(nrx)]
+    claim_outer_final, r_x = SumcheckProof.verify(fid, proof["sc_proof_outer"], 0, nrx, 3, tr)
+    cAz, cBz, cCz = (x % p for x in proof["claims_outer"])
+    eval_E, eval_W = proof["eval_E"] % p, proof["eval_W"] % p
+    if claim_outer_final != _eq_evaluate(p, tau, r_x) * (cAz * cBz - u * cCz - eval_E) % p:
+        raise ValueError("InvalidSumcheckProof")  # snark.rs:283-288
+    tr.absorb_bytes(b"claims_outer", b"".join(to_repr(x) for x in (cAz, cBz, cCz, eval_E)))
+    r = tr.squeeze(b"r")
+    claim_inner_final, r_y = SumcheckProof.verify(fid, proof["sc_proof_inner"], (cAz + r * cBz + r * r * cCz) % p,
+                                                  nry, 2, tr)
+    eval_X = _sparse_poly_evaluate(p, nry - 1, [u] + [x % p for x in U["X"]], r_y[1:])
+    eval_Z = ((1 - r_y[0]) * eval_W + r_y[0] * eval_X) % p
+    mark("sumcheck_checks")
+    T_x, T_y = DeviceVec(32 * num_cons), DeviceVec(32 << nry)
+    rx_dev, ry_dev = DeviceVec.from_bytes(fields.pack(fid, r_x)), DeviceVec.from_bytes(fields.pack(fid, r_y))
+    check(lib().b200_eq_table_dev(fid, rx_dev.ptr, nrx, T_x.ptr, None))
+    check(lib().b200_eq_table_dev(fid, ry_dev.ptr, nry, T_y.ptr, None))
+    mark("eq_tables")
+    evA, evB, evC = R1CSShape(S["A"], S["B"], S["C"]).multi_evaluate_dev(T_x, num_cons, T_y, 1 << nry)
+    mark("matrix_eval")
+    if claim_inner_final != (evA + r * evB + r * r * evC) * eval_Z % p:
+        raise ValueError("InvalidSumcheckProof")  # snark.rs:355-358
+    tr.absorb_bytes(b"w", to_repr(eval_W))
+    # batch_eval_verify (spartan/mod.rs:436-480) over the claims W(r_y[1..]) = eval_W and E(r_x) = eval_E
+    u_vec = [(U["comm_W"], r_y[1:], eval_W), (U["comm_E"], r_x, eval_E)]
+    evals_batch = [x % p for x in proof["evals_batch"]]
+    if len(evals_batch) != len(u_vec):
+        raise ValueError("InvalidInputLength")  # the reference's assert_eq (mod.rs:445)
+    rho = tr.squeeze(b"r")
+    powers = [pow(rho, i, p) for i in range(len(u_vec))]
+    num_rounds = [len(x) for (_, x, _) in u_vec]
+    nmax = max(num_rounds)
+    claim_batch_final, r_b = SumcheckProof.verify_batch(fid, proof["sc_proof_batch"], [e for (_, _, e) in u_vec],
+                                                        num_rounds, powers, 2, tr)
+    expected = sum(_eq_evaluate(p, r_b[nmax - len(x):], x) * ev * k
+                   for (_, x, _), ev, k in zip(u_vec, evals_batch, powers)) % p
+    if claim_batch_final != expected:
+        raise ValueError("InvalidSumcheckProof")  # mod.rs:471-473
+    tr.absorb_bytes(b"l", b"".join(to_repr(x) for x in evals_batch))
+    c = tr.squeeze(b"c")
+    batched_e, coeffs = 0, []
+    for i, (ev, nv) in enumerate(zip(evals_batch, num_rounds)):  # PolyEvalInstance::batch_diff_size, mod.rs:304-344
+        lag = 1
+        for rr in r_b[:nmax - nv]:
+            lag = lag * (1 - rr) % p
+        coeffs.append(pow(c, i, p))
+        batched_e = (batched_e + coeffs[i] * lag * ev) % p
+    batched_c = DlogGroup(curve).vartime_multiscalar_mul(
+        fields.pack(fid, coeffs), b"".join(_affine_bytes(curve, cm) for (cm, _, _) in u_vec))
+    mark("batch_eval_verify")
+    return batched_c, r_b, batched_e
+
+
+def verify(curve, S: dict, U: dict, vk_digest: int, proof: dict, transcript, ee: str = "ipa",
+           ck: CommitmentKey | None = None, timings: dict | None = None):
+    """The whole RelaxedR1CSSNARK::verify (snark.rs:259-396): verify_core, then EE::verify on the joint claim with the
+    same transcript.  Returns None on success (the reference's Ok(())); a failed check raises ValueError with the
+    reference's error kind (InvalidSumcheckProof, InvalidInputLength, InternalError, InvalidPCS).
+      ee = "ipa": ipa_pc.rs:80-100, 286-396; `ck` is the Pedersen key registered with h = ck_c, at least
+                  max(num_cons, num_vars) bases (checked before any device work).
+    HyperKZG and Mercury end in a pairing check, which stays with the caller: take verify_core's claim."""
+    if ee in ("hyperkzg", "mercury"):
+        raise ValueError(f"ee={ee!r}: the pairing check is not done here; run verify_core and check its claim")
+    if ee != "ipa":
+        raise ValueError(f"unknown evaluation engine {ee!r}")
+    from .ipa import check_key, verify_at_point
+    check_key(ck, max(S["num_cons"], S["num_vars"]))
+    C, x, e = verify_core(curve, S, U, vk_digest, proof, transcript, timings)
+    verify_at_point(curve, ck, C, x, e, proof["eval_arg"], transcript, timings)

@@ -131,6 +131,25 @@ class R1CSShape:
         r1, r2 = self._multi([self.A, self.B, self.C], z1, z2)
         return tuple(r1), tuple(r2)
 
+    def _handles(self):
+        return (c_u64 * 3)(self.A.handle, self.B.handle, self.C.handle)
+
+    def multi_evaluate(self, r_x: list, r_y: list) -> list:
+        """[A(r_x, r_y), B(r_x, r_y), C(r_x, r_y)] = sum over each matrix's entries of eq(r_x)[row] eq(r_y)[col] val
+        (multi_evaluate of RelaxedR1CSSNARK::verify, spartan/snark.rs:325-355).  r_x, r_y: the points as integers;
+        both eq tables are built on the device (b200_r1cs_eval)."""
+        fid = self.A.fid
+        out = ctypes.create_string_buffer(96)
+        check(lib().b200_r1cs_eval(self._handles(), 3, _cbuf(fields.pack(fid, r_x)), len(r_x),
+                                   _cbuf(fields.pack(fid, r_y)), len(r_y), out))
+        return fields.unpack(fid, out.raw)
+
+    def multi_evaluate_dev(self, T_x: "DeviceVec", tx_len: int, T_y: "DeviceVec", ty_len: int) -> list:
+        """The same on resident eq tables T_x (tx_len entries >= rows) and T_y (ty_len entries >= cols)."""
+        out = _small_buf("r1cs_eval", 96)
+        check(lib().b200_r1cs_eval_dev(self._handles(), 3, T_x.ptr, tx_len, T_y.ptr, ty_len, out.ptr, None))
+        return fields.unpack(self.A.fid, out.to_bytes(96))
+
 
 # ---------------------------------------------------------------------------------------------
 # polynomials
@@ -408,6 +427,36 @@ def update_claim(p, claim, evals, r):
 
 
 class SumcheckProof:
+    @staticmethod
+    def verify(fid, polys, claim, num_rounds, degree_bound, transcript):
+        """SumcheckProof::verify (sumcheck.rs:87-127): `polys` are the compressed round polynomials (the coefficients
+        without the linear term, CompressedUniPoly::decompress restores it from the running claim).  Returns (the
+        final claim, the challenges); a wrong number of rounds or a degree above the bound raises
+        ValueError("InvalidSumcheckProof")."""
+        p = fields.MODULUS[fid]
+        if len(polys) != num_rounds:
+            raise ValueError("InvalidSumcheckProof")
+        e, rs = claim % p, []
+        for cp in polys:
+            if not 1 <= len(cp) <= degree_bound:  # decompressed degree = len(cp); an empty message has no c0
+                raise ValueError("InvalidSumcheckProof")
+            poly = UniPoly(p, [cp[0], e - 2 * cp[0] - sum(cp[1:])] + list(cp[1:]))
+            transcript.absorb_bytes(b"p", poly.to_transcript_bytes())
+            r = transcript.squeeze(b"c")
+            rs.append(r)
+            e = poly.evaluate(r)
+        return e, rs
+
+    @staticmethod
+    def verify_batch(fid, polys, claims, num_rounds, coeffs, degree_bound, transcript):
+        """SumcheckProof::verify_batch (sumcheck.rs:131-161): instances of different sizes, each claim scaled by
+        2^(n - n_i) for the padding and combined with `coeffs`, then `verify` over n = max n_i rounds."""
+        p = fields.MODULUS[fid]
+        assert len(claims) == len(num_rounds) == len(coeffs)
+        nmax = max(num_rounds)
+        claim = sum(c * pow(2, nmax - nr, p) * k for c, nr, k in zip(claims, num_rounds, coeffs)) % p
+        return SumcheckProof.verify(fid, polys, claim, nmax, degree_bound, transcript)
+
     @staticmethod
     def prove_batch_eval(fid, claims, num_rounds, polys: list, eq_points: list, coeffs, transcript):
         """sumcheck.rs:251-351: batched evaluation claims of different sizes; polynomials resident on
